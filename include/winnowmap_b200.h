@@ -91,6 +91,10 @@ void wm_bloom_destroy(wm_bloom_t *b);
  * malloc()ed by the callee and owned by the caller (free()). */
 int wm_sketch_batch(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
                     int w, int k, wm128_t **out, int64_t **out_off);
+/* The same with is_hpc = 1 (homopolymer-compressed k-mers, src/sketch.c:146-157): positions are those of the last base
+ * of each minimizer's last homopolymer run, spans (x & 0xff) the number of bases its k runs cover. */
+int wm_sketch_batch_hpc(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
+                        int w, int k, wm128_t **out, int64_t **out_off);
 
 /* radix_sort_128x (src/misc.c:156; src/ksort.h:116-151) on n_arr independent arrays:
  * array i is a[off[i] .. off[i+1]); sorted in place with the reference's tie order. */
@@ -231,14 +235,24 @@ typedef struct wm_gpu_ctx_s wm_gpu_ctx;
  * device, or calls this once per device).  Returns NULL on an unsupported (k, w).  Call site in the reference: after
  * main.c:403 (INTEGRATION.md section 3 shows the bucket walk that fills the view). */
 wm_gpu_ctx *wm_gpu_idx_upload(const wm_idx_view_t *idx, int device);
+/* The same for an index built with flags (mm_idx_t::flag): idx_flag may carry MM_I_HPC (0x1), under which the reads are
+ * sketched homopolymer-compressed and the alignment anchors are adjusted as mm_adjust_minier does (src/align.c:350-365).
+ * Any other bit is refused (NULL).  wm_gpu_idx_upload(idx, device) is wm_gpu_idx_upload_flag(idx, 0, device). */
+wm_gpu_ctx *wm_gpu_idx_upload_flag(const wm_idx_view_t *idx, int idx_flag, int device);
+/* the index flag the context maps with (MM_I_HPC or 0) */
+int wm_idx_flag(const wm_gpu_ctx *ctx);
 void wm_gpu_destroy(wm_gpu_ctx *ctx);
 
 /* Index construction from FASTA (mm_idx_gen, src/index.c:378-449; reader loop main.c:384): the reference
  * sequences are sketched by the same CUDA kernel as the reads, the -W list goes into the down-weight filter. */
 wm_gpu_ctx *wm_index_build(const char *ref_fn, const char *kmer_freq_fn, int k, int w, int device);
+/* The same with the index options of mm_idx_reader_open (src/index.c:688): io->k, io->w and io->flag, of which only
+ * MM_I_HPC (-H, src/main.c:166) is supported; other flag bits are refused (NULL). */
+wm_gpu_ctx *wm_index_build_opt(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, int device);
 
 /* One-time index fan-out (SURVEY.md 8e): the flattened index as one relocatable blob.  Rank 0 builds it, it travels
- * GPU-to-GPU in a single NCCL broadcast, every other rank re-creates its context with wm_idx_blob_load. */
+ * GPU-to-GPU in a single NCCL broadcast, every other rank re-creates its context with wm_idx_blob_load.  The index flag
+ * travels in bits 16..31 of the second header word (zero without flags, so such a blob is byte-identical to before). */
 int64_t wm_idx_blob_size(const wm_gpu_ctx *ctx);
 int wm_idx_blob_write(const wm_gpu_ctx *ctx, uint8_t *buf);
 wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
@@ -298,7 +312,10 @@ void wm_prof_reset(void);
  * ms, ms during which at least one kernel of the class ran (launches of concurrent lanes overlap), launches, algorithmic
  * bytes (SURVEY.md 8d), units (block cells / anchors), DP jobs */
 void wm_prof_get(double *out13);
-void wm_prof_get_copies(double *out2); /* bytes copied host-to-device / device-to-host by the mapping path since wm_prof_reset */
+void wm_prof_get_copies(double *out2);
+/* the sketch stage alone (wm_sketch_batch without the copies out), plain or with is_hpc; *ms = mean CUDA-event time of
+ * one call over `reps` calls on reads already packed on the device (tools/bench_hpc.py) */
+int wm_bench_sketch(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, int w, int k, int is_hpc, int reps, double *ms); /* bytes copied host-to-device / device-to-host by the mapping path since wm_prof_reset */
 int wm_device_synchronize(void);
 int wm_device_mem(double *free_bytes, double *total_bytes); /* cudaMemGetInfo of the current device */
 void wm_dump_timers(void); /* prints and resets the orchestration wall-clock accumulators (stderr) */

@@ -302,5 +302,96 @@ def main():
         save_ref_index(name, gdir, tmp)
 
 
+# ---- homopolymer-compressed (-H) goldens: tests/golden/hpc_manifest.json and hpc_*.paf.gz; manifest.json is not touched ----
+HPC_CASES = {
+    # name: inputs (a case of CASES, or "clr": make_clr_inputs), preset, -a as well
+    "hpc_ont_small": dict(inputs="ont_small", preset="map-ont", sam=True),   # two-stage SV-aware path
+    "hpc_hifi_small": dict(inputs="hifi_small", preset="map-pb", sam=False),  # -W on compressed k-mers, tandem arrays
+    "hpc_clr": dict(inputs="clr", preset="map-pb-clr", sam=False),            # SV-aware off; planted homopolymers up to 400 bp
+}
+CLR = dict(ref_len=200000, contigs=2, ref_seed=1031, n_reads=50, n50=8000, err=0.10, read_seed=2031, min_len=1000, n_hp=120)
+
+
+def _hp_errors(rng, seq, err):
+    """Errors of an older long-read chemistry: i.i.d. errors at rate err / 2, plus homopolymer-length errors (a run
+    grows or shrinks by one or two bases) at about err / 2 per run, plus a few short N runs."""
+    s = gen_data.mutate(rng, seq, err / 2)
+    out, i, n = [], 0, len(s)
+    while i < n:
+        j = i + 1
+        while j < n and s[j] == s[i]:
+            j += 1
+        L = j - i
+        if rng.random() < err / 2:
+            L = max(1, L + int(rng.choice([-2, -1, 1, 2])))
+        out.append(np.full(L, s[i], dtype=np.uint8))
+        i = j
+    r = np.concatenate(out)
+    for _ in range(int(rng.integers(0, 3))):
+        p, m = int(rng.integers(0, len(r))), int(rng.integers(1, 20))
+        r[p:p + m] = ord("N")
+    return r
+
+
+def make_clr_inputs(outdir):
+    """A reference with planted homopolymers of 20-400 bp (some >= 256, so that spans >= 256 reach the output) and reads
+    with about 10 % errors, homopolymer-length indels and a few N runs."""
+    c = CLR
+    os.makedirs(outdir, exist_ok=True)
+    ref, reads = os.path.join(outdir, "hpc_clr.ref.fa"), os.path.join(outdir, "hpc_clr.reads.fa")
+    rng = np.random.default_rng(c["ref_seed"])
+    contigs = gen_data.make_ref(rng, c["ref_len"], c["contigs"], False)
+    planted = []
+    for name, seq in contigs:
+        seq = seq.copy()
+        for _ in range(c["n_hp"] // len(contigs)):
+            L = int(rng.integers(20, 401))
+            p = int(rng.integers(1000, len(seq) - 1000 - L))
+            seq[p:p + L] = gen_data.ACGT[int(rng.integers(0, 4))]
+        planted.append((name, seq))
+    gen_data.write_fasta(ref, planted)
+    rng = np.random.default_rng(c["read_seed"])
+    recs = gen_data.make_reads(rng, planted, c["n_reads"], c["n50"], 0.0, min_len=c["min_len"])
+    recs = [(nm, _hp_errors(rng, sq, c["err"])) for nm, sq in recs]
+    gen_data.write_fasta(reads, recs)
+    return ref, reads, None
+
+
+def make_hpc_inputs(name, outdir):
+    src = HPC_CASES[name]["inputs"]
+    return make_clr_inputs(outdir) if src == "clr" else make_inputs(src, outdir)
+
+
+def main_hpc():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_hpc"
+    manifest = {}
+    for name, c in HPC_CASES.items():
+        ref, reads, wfile = make_hpc_inputs(name, tmp)
+        base = ["-t", "4", "-H", "-x", c["preset"]] + (["-W", wfile] if wfile else [])
+        cmd = [refbin, "-c"] + base + [ref, reads]
+        out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+        with gzip.GzipFile(os.path.join(gdir, name + ".paf.gz"), "wb", mtime=0) as f:
+            f.write(out)
+        m = dict(params=dict(c, clr=CLR if c["inputs"] == "clr" else None), ref_md5=md5(ref), reads_md5=md5(reads),
+                 w_md5=md5(wfile) if wfile else None, cmd=" ".join(["winnowmap", "-c"] + base + [ref, reads]),
+                 n_lines=out.count(b"\n"), paf_md5=hashlib.md5(out).hexdigest())
+        if c["sam"]:
+            out = subprocess.run([refbin, "-a"] + base + [ref, reads], stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+            body = sam_without_pg(out)
+            with gzip.GzipFile(os.path.join(gdir, name + ".sam.stripped.gz"), "wb", mtime=0) as f:
+                f.write(sam_strip_seq(body))
+            m["sam_md5"], m["sam_lines"] = hashlib.md5(body).hexdigest(), body.count(b"\n")
+        manifest[name] = m
+        print(name, m["n_lines"], "lines")
+    json.dump(manifest, open(os.path.join(gdir, "hpc_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
-    main()
+    if "--hpc" in sys.argv:
+        main_hpc()
+    else:
+        main()

@@ -157,14 +157,22 @@ static bool kw_ok(const char *who, int k, int w)
 	return false;
 }
 
-extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload(const wm_idx_view_t *v, int device)
+// the index flags the mapping path honours (mm_idx_t::flag, src/minimap.h:41-43): only MM_I_HPC
+static bool idx_flag_ok(const char *who, int flag)
+{
+	if ((flag & ~WM_I_HPC) == 0) return true;
+	fprintf(stderr, "[ERROR] %s: index flag 0x%x not supported (only MM_I_HPC = 0x%x)\n", who, flag, WM_I_HPC);
+	return false;
+}
+
+extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload_flag(const wm_idx_view_t *v, int idx_flag, int device)
 {
 	require_device("wm_gpu_idx_upload");
-	if (!kw_ok("wm_gpu_idx_upload", v->k, v->w)) return 0;
+	if (!kw_ok("wm_gpu_idx_upload", v->k, v->w) || !idx_flag_ok("wm_gpu_idx_upload", idx_flag)) return 0;
 	wm_gpu_ctx_s *c = new wm_gpu_ctx_s();
 	memset(&c->stats, 0, sizeof(c->stats));
 	c->device = device; c->t_index = c->t_map = 0;
-	c->hidx.k = v->k, c->hidx.w = v->w;
+	c->hidx.k = v->k, c->hidx.w = v->w, c->hidx.flag = idx_flag;
 	for (int i = 0; i < v->n_seq; ++i) {
 		c->hidx.name.push_back(v->seq_name && v->seq_name[i] ? v->seq_name[i] : std::to_string(i));
 		c->hidx.len.push_back(v->seq_len[i]);
@@ -181,6 +189,9 @@ extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload(const wm_idx_view_t *v, int device)
 	return c;
 }
 
+extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload(const wm_idx_view_t *v, int device) { return wm_gpu_idx_upload_flag(v, 0, device); }
+extern "C" int wm_idx_flag(const wm_gpu_ctx_s *c) { return c->hidx.flag; }
+
 extern "C" void wm_gpu_destroy(wm_gpu_ctx_s *c)
 {
 	if (!c) return;
@@ -193,11 +204,12 @@ extern "C" void wm_gpu_destroy(wm_gpu_ctx_s *c)
 }
 
 // Index construction from a FASTA file (mm_idx_gen, src/index.c:378-449): same minimizers as the reference
-// because the reference sequences go through the same sketch kernel as the reads.
-extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_freq_fn, int k, int w, int device)
+// because the reference sequences go through the same sketch kernel as the reads.  With WM_I_HPC the minimizers are
+// those of the homopolymer-compressed sequences (mm_sketch with is_hpc, src/index.c:347); S stays uncompressed.
+static wm_gpu_ctx_s *index_build(const char *who, const char *ref_fn, const char *kmer_freq_fn, int k, int w, int idx_flag, int device)
 {
-	require_device("wm_index_build");
-	if (!kw_ok("wm_index_build", k, w)) return 0;
+	require_device(who);
+	if (!kw_ok(who, k, w) || !idx_flag_ok(who, idx_flag)) return 0;
 	WM_CUDA_CHECK(cudaSetDevice(device));
 	const double t0 = now_s();
 	SeqReader rd;
@@ -206,7 +218,7 @@ extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_fre
 	memset(&c->stats, 0, sizeof(c->stats));
 	c->device = device; c->t_index = c->t_map = 0;
 	wm_host_idx &H = c->hidx;
-	H.k = k, H.w = w;
+	H.k = k, H.w = w, H.flag = idx_flag;
 	std::vector<uint64_t> kmers;
 	if (read_kmer_list(kmer_freq_fn, k, kmers) < 0) abort();
 	wm_bloom_s *bloom = wm_bloom_build(kmers.empty() ? 0 : kmers.data(), (int64_t)kmers.size());
@@ -228,7 +240,8 @@ extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_fre
 		WM_CUDA_CHECK(cudaMemcpy(da, group.data(), group.size(), cudaMemcpyHostToDevice));
 		wm_pack_ascii(da, (int64_t)group.size(), (uint32_t*)pks.pk, (uint32_t*)pks.nm, 0);
 		int64_t n_mz = 0;
-		wm_sketch_run(&ws, bf, pks, tasks.data(), (int)tasks.size(), w, k, &n_mz, 0);
+		if (idx_flag & WM_I_HPC) wm_sketch_run_hpc(&ws, bf, pks, tasks.data(), (int)tasks.size(), w, k, &n_mz, 0);
+		else wm_sketch_run(&ws, bf, pks, tasks.data(), (int)tasks.size(), w, k, &n_mz, 0);
 		WM_CUDA_CHECK(cudaDeviceSynchronize());
 		if (n_mz > 0) {
 			wm128_dev *part = wm_dev_alloc<wm128_dev>(n_mz);
@@ -268,6 +281,16 @@ extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_fre
 	wm_bloom_destroy(bloom);
 	c->t_index = now_s() - t0;
 	return c;
+}
+
+extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_freq_fn, int k, int w, int device)
+{
+	return index_build("wm_index_build", ref_fn, kmer_freq_fn, k, w, 0, device);
+}
+
+extern "C" wm_gpu_ctx_s *wm_index_build_opt(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, int device)
+{
+	return index_build("wm_index_build_opt", ref_fn, kmer_freq_fn, io->k, io->w, io->flag, device);
 }
 
 extern "C" int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo) { return set_opt(preset, io, mo); }
@@ -693,7 +716,7 @@ extern "C" int wm_idx_blob_write(const wm_gpu_ctx_s *c_, uint8_t *buf)
 	size_t names = 0;
 	for (auto &s : H.name) names += s.size() + 1;
 	uint64_t *h = (uint64_t*)buf;
-	h[0] = 0x31584449424d57ULL; /* "WMBIDX1" */ h[1] = (uint64_t)H.k << 32 | (uint32_t)H.w; h[2] = H.len.size(); h[3] = names;
+	h[0] = 0x31584449424d57ULL; /* "WMBIDX1" */ h[1] = (uint64_t)H.k << 32 | (uint64_t)(uint16_t)H.flag << 16 | (uint32_t)H.w; h[2] = H.len.size(); h[3] = names;
 	h[4] = H.S.size(); h[5] = c->keys.size(); h[6] = c->pos.size(); h[7] = c->bloom_bits;
 	uint8_t *p = buf + 64;
 	memcpy(p, H.len.data(), H.len.size() * 4); p += pad8(H.len.size() * 4);
@@ -734,8 +757,9 @@ extern "C" wm_gpu_ctx_s *wm_idx_blob_load(const uint8_t *buf, int64_t size, int 
 		name_ptr[i] = nm; nm = (const char*)z + 1;
 	}
 	wm_idx_view_t v;
-	v.k = (int32_t)(h[1] >> 32), v.w = (int32_t)(uint32_t)h[1], v.n_seq = (int32_t)n_seq;
+	// h[1]: k << 32 | flag << 16 | w (w < 256; a blob without flags has zeros there)
+	v.k = (int32_t)(h[1] >> 32), v.w = (int32_t)(h[1] & 0xffff), v.n_seq = (int32_t)n_seq;
 	v.seq_name = name_ptr.data(), v.seq_len = len, v.seq_offset = off, v.S = S, v.S_words = s_words;
 	v.n_keys = (int64_t)n_keys, v.keys = keys, v.pos_off = pos_off, v.pos = pos, v.bloom_bits = h[7], v.bloom_table = p;
-	return wm_gpu_idx_upload(&v, device);
+	return wm_gpu_idx_upload_flag(&v, (int)(h[1] >> 16 & 0xffff), device);
 }

@@ -98,6 +98,7 @@ struct GpuBackendImpl {
 	wm_dbuf nc_buf, scan_tmp, coop_ids, g_jobs, g_joff, seq_pool, dp_jobs, bt, ez, cig, cig_off, cig_out, ll_jobs, ll_scr, ll_out, mat;
 	// host result pools
 	std::vector<uint32_t> h_mzpos; std::vector<int64_t> h_mz_off; std::vector<int32_t> h_rep;
+	std::vector<uint8_t> h_mzspan; wm_dbuf mz_span; // HPC index only: the minimizers' spans
 	wm_hbuf<uint64_t> h_u; wm_hbuf<wm_pair_t> h_b; std::vector<int32_t> h_nu; std::vector<int64_t> h_nb; // (the big ones: page-locked)
 	wm_hbuf<uint32_t> h_cig; wm_hbuf<wm_extz_dev> h_ez; wm_hbuf<int32_t> h_zd; wm_dbuf zd;
 	size_t bt_budget;
@@ -233,13 +234,19 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 	wm_seed_ws *sdp[2] = { &g.sd, 0 };
 	sdp[1] = &g.sd2; // second seed workspace for the masked pass (kept until chaining is done)
 	std::vector<uint32_t> pass_mzpos[2]; std::vector<int64_t> pass_mzoff[2];
+	const bool hpc = (g.hidx->flag & WM_I_HPC) != 0;
+	std::vector<uint8_t> pass_mzspan[2];
 	for (int pass = 0; pass < 2; ++pass) {
 		std::vector<wm_sk_task> &skt = pass == 0 ? skt_plain : skt_mask;
 		std::vector<int> &ids = pass == 0 ? plain_ids : mask_ids;
 		const int ns = (int)skt.size();
 		if (ns == 0) continue;
 		int64_t n_mz = 0;
-		{ WM_TIMED("seed.sketch"); wm_sketch_run(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st); }
+		{
+			WM_TIMED("seed.sketch");
+			if (hpc) wm_sketch_run_hpc(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st);
+			else wm_sketch_run(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st);
+		}
 		WM_TIMED("seed.lookup_sort");
 		std::vector<int32_t> qlen(ns);
 		for (int i = 0; i < ns; ++i) qlen[i] = skt[i].len;
@@ -254,6 +261,12 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 		WM_CUDA_CHECK(wm_memcpy_async(rep.data(), sdp[pass]->rep_len.p, sizeof(int32_t) * ns, cudaMemcpyDeviceToHost, st));
 		WM_CUDA_CHECK(wm_memcpy_async(pass_mzoff[pass].data(), g.sk.mz_off.p, sizeof(int64_t) * (ns + 1), cudaMemcpyDeviceToHost, st));
 		if (n_mz > 0) WM_CUDA_CHECK(wm_memcpy_async(pass_mzpos[pass].data(), sdp[pass]->mini_pos.p, sizeof(uint32_t) * n_mz, cudaMemcpyDeviceToHost, st));
+		if (hpc && n_mz > 0) { // the spans vary: mm_est_err averages them (src/esterr.c:37-39)
+			uint8_t *d_sp = (uint8_t*)g.mz_span.need(n_mz);
+			wm_mz_spans((const wm128_dev*)g.sk.mz.p, n_mz, d_sp, st);
+			pass_mzspan[pass].resize(n_mz);
+			WM_CUDA_CHECK(wm_memcpy_async(pass_mzspan[pass].data(), d_sp, n_mz, cudaMemcpyDeviceToHost, st));
+		}
 		wm_stream_sync(st);
 		for (int i = 0; i < ns; ++i) {
 			const int t = ids[i];
@@ -358,10 +371,16 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 	g.h_mzpos.resize(g.h_mz_off[n] + 1);
 	for (int i = 0; i < n; ++i)
 		if (mz_cnt[i] > 0) memcpy(&g.h_mzpos[g.h_mz_off[i]], &pass_mzpos[seed_pass[i]][mz_src[i]], sizeof(uint32_t) * mz_cnt[i]);
+	if (hpc) {
+		g.h_mzspan.resize(g.h_mz_off[n] + 1);
+		for (int i = 0; i < n; ++i)
+			if (mz_cnt[i] > 0) memcpy(&g.h_mzspan[g.h_mz_off[i]], &pass_mzspan[seed_pass[i]][mz_src[i]], mz_cnt[i]);
+	}
 	for (int i = 0; i < n; ++i) {
 		SeedOut &o = out[i];
 		o.rep_len = g.h_rep[i];
 		o.n_mz = (int32_t)mz_cnt[i], o.mz_pos = g.h_mzpos.data() + g.h_mz_off[i];
+		o.mz_span = hpc ? g.h_mzspan.data() + g.h_mz_off[i] : 0;
 		o.n_u = g.h_nu[i], o.u = g.h_u.data() + nu_off[i];
 		o.n_b = g.h_nb[i], o.b = g.h_b.data() + nb_off[i];
 	}

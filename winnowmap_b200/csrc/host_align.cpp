@@ -373,10 +373,28 @@ void AlignTask::init(const wm_mapopt_t *opt_, const wm_host_idx *mi_, int task_i
 	phase = 0; cur = 0; sub = 0; inv_job = -1;
 }
 
-static inline void adjust_minier(int k, const wm_pair_t *p, int32_t *r, int32_t *q)
-{ // mm_adjust_minier :350-363 without HPC
-	*r = (int32_t)p->x - (k >> 1);
-	*q = (int32_t)p->y - (k >> 1);
+static inline void adjust_minier(const wm_host_idx *mi, const uint8_t *const qseq0[2], const wm_pair_t *p, int32_t *r, int32_t *q)
+{ // mm_adjust_minier :350-365
+	if (mi->flag & WM_I_HPC) {
+		// the query walks back to the start of its homopolymer; as in the reference the loop never tests base 0
+		const uint8_t *qseq = qseq0[p->x >> 63];
+		int32_t i, c;
+		*q = (int32_t)p->y;
+		for (i = *q - 1, c = qseq[*q]; i > 0; --i)
+			if (qseq[i] != c) break;
+		*q = i + 1;
+		// mm_get_hplen_back (:341-348): the reference's run down to the contig's first base inclusive
+		const uint32_t rid = (uint32_t)(p->x << 1 >> 33);
+		const int64_t off0 = (int64_t)mi->offset[rid], off = off0 + (uint32_t)p->x;
+		const int cr = mi->base((uint64_t)off);
+		int64_t j;
+		for (j = off - 1; j >= off0; --j)
+			if (mi->base((uint64_t)j) != cr) break;
+		*r = (int32_t)p->x + 1 - (int32_t)(off - j);
+	} else {
+		*r = (int32_t)p->x - (mi->k >> 1);
+		*q = (int32_t)p->y - (mi->k >> 1);
+	}
 }
 
 // everything mm_align1 decides before its first DP (:565-688), plus the speculative job list
@@ -396,8 +414,8 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 	else as1 = r->as, cnt1 = r->cnt;
 	filter_bad_seeds(as1, cnt1, a, 10, 40, opt->max_gap >> 1, 10);
 	filter_bad_seeds_alt(as1, cnt1, a, 30, opt->max_gap >> 1);
-	adjust_minier(mi->k, &a[as1], &rs, &qs);
-	adjust_minier(mi->k, &a[as1 + cnt1 - 1], &re, &qe);
+	adjust_minier(mi, q_strand, &a[as1], &rs, &qs);
+	adjust_minier(mi, q_strand, &a[as1 + cnt1 - 1], &re, &qe);
 	A.as1 = as1, A.cnt1 = cnt1;
 	// DP region (:613-684)
 	rs0 = (int32_t)a[r->as].x + 1 - (int32_t)(a[r->as].y >> 32 & 0xff);
@@ -474,7 +492,7 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 	// gap filling windows (:709-730); they depend on the anchors only
 	for (i = 1; i < cnt1; ++i) {
 		if ((a[as1 + i].y & (WM_SEED_IGNORE | WM_SEED_TANDEM)) && i != cnt1 - 1) continue;
-		adjust_minier(mi->k, &a[as1 + i], &re, &qe);
+		adjust_minier(mi, q_strand, &a[as1 + i], &re, &qe);
 		if (i == cnt1 - 1 || (a[as1 + i].y & WM_SEED_LONG_JOIN) || (qe - qs >= opt->min_ksw_len && re - rs >= opt->min_ksw_len)) {
 			Align1::Gap g;
 			g.i = i, g.rs = rs, g.qs = qs, g.re = re, g.qe = qe, g.bw1 = bw;

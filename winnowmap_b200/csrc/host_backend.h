@@ -32,6 +32,7 @@ struct ChainParams { // arguments of mm_chain_dp (src/chain.c:22)
 struct SeedOut { // views into backend-owned host buffers, valid until the next seed_chain call
 	int32_t rep_len;
 	int32_t n_mz; const uint32_t *mz_pos; // per query minimizer: position | kept << 31 (kept == passed the occurrence filter)
+	const uint8_t *mz_span;               // per query minimizer: its span, with an HPC index only (else null: every span is k)
 	int32_t n_u; const uint64_t *u;       // score << 32 | count per chain
 	int64_t n_b; const wm_pair_t *b;      // chained anchors, chains concatenated
 };

@@ -209,7 +209,7 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 			M.mini_pos.clear();
 			if (M.est_err)
 				for (int k = 0; k < o.n_mz; ++k)
-					if (o.mz_pos[k] >> 31) M.mini_pos.push_back((uint64_t)mi->k << 32 | (o.mz_pos[k] & 0x7fffffffu));
+					if (o.mz_pos[k] >> 31) M.mini_pos.push_back((uint64_t)(o.mz_span ? o.mz_span[k] : mi->k) << 32 | (o.mz_pos[k] & 0x7fffffffu));
 			M.hash = rd->name.empty() ? 0 : x31_hash(rd->name.c_str()); // src/map.c:358-360
 			M.hash ^= wang_hash((uint32_t)M.win.wl) + wang_hash((uint32_t)M.opt->seed);
 			M.hash = wang_hash(M.hash);

@@ -59,6 +59,7 @@ typedef wm128_t wm_pair_t; // mm128_t
 // Host copy of what the path needs from the index (mm_idx_t / mm_idx_seq_t, src/minimap.h:59-77)
 struct wm_host_idx {
 	int k, w;
+	int flag = 0;            // mm_idx_t::flag: WM_I_HPC when the index holds homopolymer-compressed minimizers
 	std::vector<std::string> name;
 	std::vector<uint32_t> len;
 	std::vector<uint64_t> offset;

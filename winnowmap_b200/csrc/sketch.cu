@@ -23,6 +23,7 @@
 #include "scan.cuh"
 #include "sketch.cuh"
 #include "pkseq.cuh"
+#include "hpc.cuh"
 
 #define WM_SK_TN 1024      // new positions per tile in pass A
 #define WM_SK_THREADS 256
@@ -73,10 +74,13 @@ __device__ __forceinline__ double wm_weight(uint64_t kmer, const wm_bloom_dev &b
 #define WM_SK_PKW 96                // packed words staged per tile (64-base aligned start, + the window's look-ahead)
 #define WM_SK_SMEM (3 * WM_SK_NE * 8 + WM_SK_PKW * 4 + WM_SK_PKW * 2)
 
+// HPC: the sequence is a compressed slice (symbols), pos maps each symbol to the last base of its run (relative to the
+// uncompressed task); a k-mer whose span pos[p] - pos[p - k] reaches 256 is valid but never a candidate: key 3.0.
+template <bool HPC>
 __global__ void __launch_bounds__(WM_SK_THREADS)
 wm_sketch_order_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ tile_off,
                        const int64_t *__restrict__ base_off, int n_tasks, int w, int k, wm_bloom_dev bf,
-                       double *__restrict__ ord, uint8_t *__restrict__ elig)
+                       double *__restrict__ ord, uint8_t *__restrict__ elig, const int32_t *__restrict__ pos)
 {
 	extern __shared__ __align__(16) uint8_t sm_raw[];
 	double *s_ord = (double*)sm_raw;                 // position p0 - w + j
@@ -111,7 +115,11 @@ wm_sketch_order_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks,
 			if (!(wm_pk_nwindow(s_nm, rel) & kmask)) {
 				uint64_t f, r;
 				wm_pk_kmer(wm_pk_window(s_pk, rel), k, &f, &r);
-				if (f != r) o = wm_weight(f < r ? f : r, bf);
+				if (HPC) {
+					const int64_t q = T.seq_off + p;
+					const int span = pos[q] - (p >= k ? pos[q - k] : -1);
+					if (f != r) o = span < 256 ? wm_weight(f < r ? f : r, bf) : 3.0;
+				} else if (f != r) o = wm_weight(f < r ? f : r, bf);
 			}
 		}
 		s_ord[j] = o;
@@ -140,6 +148,8 @@ wm_sketch_order_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks,
 }
 
 // ---- pass B ----
+// v counts the valid k-mers in a row (l >= k of src/sketch.c): keys below 2.0, and under HPC also the 3.0 of pass A
+template <bool HPC>
 __global__ void wm_sketch_winnow_kernel(const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ chunk_off,
                                         const int64_t *__restrict__ base_off, int n_tasks, int64_t n_chunks, int w,
                                         const double *__restrict__ ord_all, const uint8_t *__restrict__ elig_all, uint8_t *__restrict__ flag_all)
@@ -163,14 +173,14 @@ __global__ void wm_sketch_winnow_kernel(const wm_sk_task *__restrict__ tasks, co
 		while (s < c1 && !elig[s]) ++s;
 		if (s >= c1) return; // an earlier thread runs through this chunk
 		min_i = s, min_ord = ord[s];
-		for (int j = s; j >= 0 && v < w + 1 && ord[j] < 2.0; --j) ++v;
+		for (int j = s; j >= 0 && v < w + 1 && (HPC ? ord[j] != 2.0 : ord[j] < 2.0); --j) ++v;
 		i = s + 1;
 	}
 	bool seen = false; // an eligible position was already met in the chunk that contains i
 	for (; i < len; ++i) {
 		if ((i & (WM_SK_CH - 1)) == 0) seen = false;
 		const double o = ord[i];
-		v = o < 2.0 ? (v < w + 1 ? v + 1 : v) : 0;
+		v = (HPC ? o != 2.0 : o < 2.0) ? (v < w + 1 ? v + 1 : v) : 0;
 		if (o < min_ord) { // a new minimum (src/sketch.c:180-189)
 			if (v >= w + 1 && min_i >= 0) flag[min_i] = 1;
 			min_i = i, min_ord = o;
@@ -193,8 +203,10 @@ __global__ void wm_sketch_winnow_kernel(const wm_sk_task *__restrict__ tasks, co
 }
 
 // sequential pass for even k (symmetric k-mers make ring slots != bases): one thread per sequence
+template <bool HPC>
 __global__ void wm_sketch_seq_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ base_off,
-                                     int n_tasks, int w, int k, wm_bloom_dev bf, uint8_t *__restrict__ flag_all, double *__restrict__ ring_all)
+                                     int n_tasks, int w, int k, wm_bloom_dev bf, uint8_t *__restrict__ flag_all, double *__restrict__ ring_all,
+                                     const int32_t *__restrict__ pos)
 {
 	const int tid = blockIdx.x * blockDim.x + threadIdx.x;
 	if (tid >= n_tasks) return;
@@ -215,7 +227,8 @@ __global__ void wm_sketch_seq_kernel(const wm_pkseq seq, const wm_sk_task *__res
 			kmer1 = (kmer1 >> 2) | (3ULL ^ (uint64_t)c) << shift1;
 			if (kmer0 == kmer1) continue; // src/sketch.c:166
 			++l;
-			if (l >= k) o = wm_weight(kmer0 < kmer1 ? kmer0 : kmer1, bf), oi = i;
+			if (l >= k && (!HPC || pos[T.seq_off + i] - (i >= k ? pos[T.seq_off + i - k] : -1) < 256))
+				o = wm_weight(kmer0 < kmer1 ? kmer0 : kmer1, bf), oi = i;
 		} else l = 0;
 		buf_ord[buf_pos] = o, buf_pos_[buf_pos] = (double)oi;
 		if (o < min_ord) {
@@ -249,10 +262,12 @@ __global__ void wm_sketch_count_kernel(const wm_sk_task *__restrict__ tasks, con
 	cnt[ch] = n;
 }
 
+// HPC: positions and spans come from the symbol -> base map
+template <bool HPC>
 __global__ void wm_sketch_emit_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ chunk_off,
                                       const int64_t *__restrict__ base_off, int n_tasks, int64_t n_chunks, int k,
                                       const uint8_t *__restrict__ flag_all, const int64_t *__restrict__ rank, wm128_dev *__restrict__ out,
-                                      int64_t *__restrict__ mz_off)
+                                      int64_t *__restrict__ mz_off, const int32_t *__restrict__ pos)
 {
 	const int64_t ch = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if (ch > n_chunks) return;
@@ -274,8 +289,15 @@ __global__ void wm_sketch_emit_kernel(const wm_pkseq seq, const wm_sk_task *__re
 			wm_pk_kmer(wm_pk_window(seq.pk, T.seq_off + i - (k - 1)), k, &f, &r);
 			const int z = f < r ? 0 : 1; // src/sketch.c:167
 			wm128_dev m;
-			m.x = wm_hash64(z ? r : f, mask) << 8 | (uint64_t)k;   // :171 (span == k once l >= k)
-			m.y = (uint64_t)T.rid << 32 | (uint32_t)i << 1 | (uint64_t)z; // :172
+			if (HPC) {
+				const int64_t q = T.seq_off + i;
+				const int span = pos[q] - (i >= k ? pos[q - k] : -1);
+				m.x = wm_hash64(z ? r : f, mask) << 8 | (uint64_t)span;
+				m.y = (uint64_t)T.rid << 32 | (uint32_t)pos[q] << 1 | (uint64_t)z;
+			} else {
+				m.x = wm_hash64(z ? r : f, mask) << 8 | (uint64_t)k;   // :171 (span == k once l >= k)
+				m.y = (uint64_t)T.rid << 32 | (uint32_t)i << 1 | (uint64_t)z; // :172
+			}
 			out[o++] = m;
 		}
 }
@@ -372,9 +394,11 @@ void wm_pack_gather(const char *d_pool, const int64_t *d_src_off, const int64_t 
 
 // ---- host-side launcher on device-resident code arrays ----
 // tasks (host copy) describe slices of the packed pool `seq` (offsets in bases).  On return *n_mz is the total number of minimizers,
-// ws->mz holds them (device) and ws->mz_off (device, n_tasks+1) their per-task offsets.
-void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                   int w, int k, int64_t *n_mz, cudaStream_t st)
+// ws->mz holds them (device) and ws->mz_off (device, n_tasks+1) their per-task offsets.  HPC: `seq` is the compressed pool and
+// `pos` its symbol -> base map (wm_sketch_run_hpc).
+template <bool HPC>
+static void wm_sketch_passes(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
+                             int w, int k, const int32_t *pos, int64_t *n_mz, cudaStream_t st)
 {
 	*n_mz = 0;
 	std::vector<int64_t> h_off(3 * (size_t)(n_tasks + 1));
@@ -400,13 +424,13 @@ void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq
 	if (k & 1) {
 		double *d_ord = (double*)ws->ord.need(sizeof(double) * n_bases);
 		uint8_t *d_elig = (uint8_t*)ws->elig.need(n_bases);
-		wm_count_launch(); wm_sketch_order_kernel<<<(unsigned)n_tiles, WM_SK_THREADS, WM_SK_SMEM, st>>>(seq, d_tasks, d_tile_off, d_base_off, n_tasks, w, k, bf, d_ord, d_elig);
+		wm_count_launch(); wm_sketch_order_kernel<HPC><<<(unsigned)n_tiles, WM_SK_THREADS, WM_SK_SMEM, st>>>(seq, d_tasks, d_tile_off, d_base_off, n_tasks, w, k, bf, d_ord, d_elig, pos);
 		WM_CUDA_CHECK(cudaGetLastError());
-		wm_count_launch(); wm_sketch_winnow_kernel<<<(unsigned)((n_chunks + 127) / 128), 128, 0, st>>>(d_tasks, d_chunk_off, d_base_off, n_tasks, n_chunks, w, d_ord, d_elig, d_flag);
+		wm_count_launch(); wm_sketch_winnow_kernel<HPC><<<(unsigned)((n_chunks + 127) / 128), 128, 0, st>>>(d_tasks, d_chunk_off, d_base_off, n_tasks, n_chunks, w, d_ord, d_elig, d_flag);
 		WM_CUDA_CHECK(cudaGetLastError());
 	} else {
 		double *d_ring = (double*)ws->ord.need(sizeof(double) * 512 * (size_t)n_tasks);
-		wm_count_launch(); wm_sketch_seq_kernel<<<(n_tasks + 63) / 64, 64, 0, st>>>(seq, d_tasks, d_base_off, n_tasks, w, k, bf, d_flag, d_ring);
+		wm_count_launch(); wm_sketch_seq_kernel<HPC><<<(n_tasks + 63) / 64, 64, 0, st>>>(seq, d_tasks, d_base_off, n_tasks, w, k, bf, d_flag, d_ring, pos);
 		WM_CUDA_CHECK(cudaGetLastError());
 	}
 	int32_t *d_cnt = (int32_t*)ws->cnt.need(sizeof(int32_t) * (n_chunks + 1));
@@ -424,10 +448,136 @@ void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq
 		std::vector<int64_t> fill(n_tasks + 1, total);
 		WM_CUDA_CHECK(wm_memcpy_async(d_mz_off, fill.data(), sizeof(int64_t) * (n_tasks + 1), cudaMemcpyHostToDevice, st));
 	}
-	wm_count_launch(); wm_sketch_emit_kernel<<<(unsigned)((n_chunks + 1 + 127) / 128), 128, 0, st>>>(seq, d_tasks, d_chunk_off, d_base_off, n_tasks, n_chunks, k,
-	                                                                               d_flag, d_rank, d_mz, d_mz_off);
+	wm_count_launch(); wm_sketch_emit_kernel<HPC><<<(unsigned)((n_chunks + 1 + 127) / 128), 128, 0, st>>>(seq, d_tasks, d_chunk_off, d_base_off, n_tasks, n_chunks, k,
+	                                                                                    d_flag, d_rank, d_mz, d_mz_off, pos);
 	WM_CUDA_CHECK(cudaGetLastError());
 	*n_mz = total;
+}
+
+void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
+                   int w, int k, int64_t *n_mz, cudaStream_t st)
+{
+	wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st);
+}
+
+// ---- homopolymer-compressed sketch: a compaction front end, then the passes above on the compressed slices ----
+// H1: one thread per 32-base group of a task: the symbol ends of the group (hpc.cuh) and their number
+__global__ void wm_hpc_mark_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ grp_off, int n_tasks,
+                                   int64_t n_groups, uint32_t *__restrict__ ends, int32_t *__restrict__ cnt)
+{
+	const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n_groups) return;
+	int lo = 0, hi = n_tasks;
+	while (hi - lo > 1) { int m = (lo + hi) >> 1; if (grp_off[m] <= g) lo = m; else hi = m; }
+	const wm_sk_task T = tasks[lo];
+	const int j = (int)(g - grp_off[lo]);
+	const int64_t b = T.seq_off + 32 * (int64_t)j;
+	uint32_t e = wm_hpc_ends32(wm_pk_window(seq.pk, b), wm_pk_window(seq.pk, b + 1), wm_pk_nwindow(seq.nm, b), wm_pk_nwindow(seq.nm, b + 1));
+	e = wm_hpc_clip(e, j, T.len);
+	ends[g] = e, cnt[g] = __popc(e);
+}
+
+// H3: every symbol's base (relative to its task) at its rank; coff[t] = the first symbol of task t (coff[n_tasks] = total)
+__global__ void wm_hpc_scatter_kernel(const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ grp_off, int n_tasks, int64_t n_groups,
+                                      const uint32_t *__restrict__ ends, const int64_t *__restrict__ rank, int32_t *__restrict__ pos,
+                                      int64_t *__restrict__ coff)
+{
+	const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (g > n_groups) return;
+	if (g == n_groups) { // the total, also for trailing empty tasks
+		coff[n_tasks] = rank[n_groups];
+		for (int t = n_tasks - 1; t >= 0 && tasks[t].len <= 0; --t) coff[t] = rank[n_groups];
+		return;
+	}
+	int lo = 0, hi = n_tasks;
+	while (hi - lo > 1) { int m = (lo + hi) >> 1; if (grp_off[m] <= g) lo = m; else hi = m; }
+	const int j = (int)(g - grp_off[lo]);
+	int64_t o = rank[g];
+	if (j == 0) { // empty tasks own no group: give them the offset of the next non-empty one
+		coff[lo] = o;
+		for (int t = lo - 1; t >= 0 && tasks[t].len <= 0; --t) coff[t] = o;
+	}
+	for (uint32_t e = ends[g]; e; e &= e - 1) pos[o++] = 32 * j + __ffs(e) - 1;
+}
+
+// H4: the compressed pool, one thread per 32 symbols (the gather of wm_pack_gather_kernel, symbol s of task t being base
+// pos[s] of the task); past the last symbol the codes read as ambiguous
+__global__ void __launch_bounds__(256)
+wm_hpc_pack_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ coff, int n_tasks,
+                   const int32_t *__restrict__ pos, int64_t n, uint32_t *__restrict__ pk, uint32_t *__restrict__ nm)
+{
+	const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, s0 = g * 32;
+	if (s0 >= n) return;
+	int lo = 0, hi = n_tasks;
+	while (hi - lo > 1) { const int m = (lo + hi) >> 1; if (coff[m] <= s0) lo = m; else hi = m; }
+	uint64_t p = 0; uint32_t m = 0;
+	for (int j = 0; j < 32; ++j) {
+		const int64_t s = s0 + j;
+		int c = 4;
+		if (s < n) {
+			while (s >= coff[lo + 1]) ++lo;
+			c = wm_pk_get(seq, tasks[lo].seq_off + pos[s]);
+		}
+		p |= (uint64_t)(c & 3) << 2 * j;
+		m |= (uint32_t)(c >> 2) << j;
+	}
+	((uint2*)pk)[g] = make_uint2((uint32_t)p, (uint32_t)(p >> 32));
+	nm[g] = m;
+}
+
+void wm_sketch_run_hpc(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
+                       int w, int k, int64_t *n_mz, cudaStream_t st)
+{
+	*n_mz = 0;
+	std::vector<int64_t> grp_off(n_tasks + 1, 0);
+	for (int i = 0; i < n_tasks; ++i) grp_off[i + 1] = grp_off[i] + (h_tasks[i].len > 0 ? (h_tasks[i].len + 31) / 32 : 0);
+	const int64_t n_groups = grp_off[n_tasks];
+	if (n_tasks == 0 || n_groups == 0) { wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st); return; }
+	wm_sk_task *d_tasks = (wm_sk_task*)ws->hpc_tasks.need(sizeof(wm_sk_task) * n_tasks);
+	int64_t *d_goff = (int64_t*)ws->hpc_goff.need(sizeof(int64_t) * (n_tasks + 1));
+	int64_t *d_coff = (int64_t*)ws->hpc_coff.need(sizeof(int64_t) * (n_tasks + 1));
+	uint32_t *d_ends = (uint32_t*)ws->hpc_ends.need(sizeof(uint32_t) * n_groups);
+	int32_t *d_cnt = (int32_t*)ws->cnt.need(sizeof(int32_t) * (n_groups + 1));
+	int64_t *d_rank = (int64_t*)ws->rank.need(sizeof(int64_t) * (n_groups + 2));
+	int64_t *d_tmp = (int64_t*)ws->scan_tmp.need(sizeof(int64_t) * wm_scan_tmp_elems(n_groups));
+	WM_CUDA_CHECK(wm_memcpy_async(d_tasks, h_tasks, sizeof(wm_sk_task) * n_tasks, cudaMemcpyHostToDevice, st));
+	WM_CUDA_CHECK(wm_memcpy_async(d_goff, grp_off.data(), sizeof(int64_t) * (n_tasks + 1), cudaMemcpyHostToDevice, st));
+	wm_count_launch(); wm_hpc_mark_kernel<<<(unsigned)((n_groups + 127) / 128), 128, 0, st>>>(seq, d_tasks, d_goff, n_tasks, n_groups, d_ends, d_cnt);
+	WM_CUDA_CHECK(cudaGetLastError());
+	wm_exclusive_scan(d_cnt, n_groups, d_rank, d_tmp, st);
+	int64_t n_sym = 0;
+	WM_CUDA_CHECK(wm_memcpy_async(&n_sym, d_rank + n_groups, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+	wm_stream_sync(st);
+	int32_t *d_pos = (int32_t*)ws->hpc_pos.need(sizeof(int32_t) * (n_sym + 1));
+	wm_count_launch(); wm_hpc_scatter_kernel<<<(unsigned)((n_groups + 1 + 127) / 128), 128, 0, st>>>(d_tasks, d_goff, n_tasks, n_groups, d_ends, d_rank, d_pos, d_coff);
+	WM_CUDA_CHECK(cudaGetLastError());
+	wm_pkseq cs;
+	cs.pk = (const uint32_t*)ws->hpc_pk.need(sizeof(uint32_t) * wm_pk_words(n_sym));
+	cs.nm = (const uint32_t*)ws->hpc_nm.need(sizeof(uint32_t) * wm_nm_words(n_sym));
+	wm_pack_tail(n_sym, (uint32_t*)cs.pk, (uint32_t*)cs.nm, st);
+	wm_count_launch(); wm_hpc_pack_kernel<<<(unsigned)((n_sym + 32 * 256 - 1) / (32 * 256)), 256, 0, st>>>(seq, d_tasks, d_coff, n_tasks, d_pos, n_sym,
+	                                                                                                   (uint32_t*)cs.pk, (uint32_t*)cs.nm);
+	WM_CUDA_CHECK(cudaGetLastError());
+	std::vector<int64_t> coff(n_tasks + 1);
+	WM_CUDA_CHECK(wm_memcpy_async(coff.data(), d_coff, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyDeviceToHost, st));
+	wm_stream_sync(st);
+	std::vector<wm_sk_task> ct(n_tasks);
+	for (int i = 0; i < n_tasks; ++i) ct[i].seq_off = coff[i], ct[i].len = (int32_t)(coff[i + 1] - coff[i]), ct[i].rid = h_tasks[i].rid;
+	wm_sketch_passes<true>(ws, bf, cs, ct.data(), n_tasks, w, k, d_pos, n_mz, st);
+}
+
+// one byte per minimizer: its span (x & 0xff)
+__global__ void wm_mz_span_kernel(const wm128_dev *__restrict__ mz, int64_t n, uint8_t *__restrict__ span)
+{
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) span[i] = (uint8_t)(mz[i].x & 0xff);
+}
+
+void wm_mz_spans(const wm128_dev *d_mz, int64_t n, uint8_t *d_span, cudaStream_t st)
+{
+	if (n <= 0) return;
+	wm_count_launch(); wm_mz_span_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_mz, n, d_span);
+	WM_CUDA_CHECK(cudaGetLastError());
 }
 
 // ---- down-weight filter construction (host; replaces bloom_filter of src/index.c:404-432) ----
@@ -490,8 +640,8 @@ void wm_bloom_dev_from_table(wm_bloom_dev *d, const uint8_t *d_table, uint64_t b
 }
 
 // ---- C ABI: batched mm_sketch ----
-extern "C" int wm_sketch_batch(const wm_bloom_s *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
-                               int w, int k, wm128_dev **out, int64_t **out_off)
+static int wm_sketch_batch_impl(const wm_bloom_s *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
+                                int w, int k, int is_hpc, wm128_dev **out, int64_t **out_off)
 {
 	int ndev = 0;
 	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
@@ -518,11 +668,61 @@ extern "C" int wm_sketch_batch(const wm_bloom_s *bloom, int n, const char *seq, 
 	for (int i = 0; i < n; ++i) tasks[i].seq_off = off[i], tasks[i].len = (int32_t)(off[i + 1] - off[i]), tasks[i].rid = rid ? rid[i] : 0;
 	wm_sketch_ws ws;
 	int64_t n_mz = 0;
-	wm_sketch_run(&ws, bf, pks, tasks.data(), n, w, k, &n_mz, 0);
+	if (is_hpc) wm_sketch_run_hpc(&ws, bf, pks, tasks.data(), n, w, k, &n_mz, 0);
+	else wm_sketch_run(&ws, bf, pks, tasks.data(), n, w, k, &n_mz, 0);
 	WM_CUDA_CHECK(cudaDeviceSynchronize());
 	*out = (wm128_dev*)malloc(sizeof(wm128_dev) * (n_mz > 0 ? n_mz : 1));
 	if (n_mz > 0) WM_CUDA_CHECK(cudaMemcpy(*out, ws.mz.p, sizeof(wm128_dev) * n_mz, cudaMemcpyDeviceToHost));
 	WM_CUDA_CHECK(cudaMemcpy(*out_off, ws.mz_off.p, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost));
+	ws.release();
+	cudaFree(d_ascii); cudaFree(d_pk); cudaFree(d_nm); cudaFree(d_table);
+	return 0;
+}
+
+extern "C" int wm_sketch_batch(const wm_bloom_s *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
+                               int w, int k, wm128_dev **out, int64_t **out_off)
+{
+	return wm_sketch_batch_impl(bloom, n, seq, off, rid, w, k, 0, out, out_off);
+}
+
+extern "C" int wm_sketch_batch_hpc(const wm_bloom_s *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
+                                   int w, int k, wm128_dev **out, int64_t **out_off)
+{
+	return wm_sketch_batch_impl(bloom, n, seq, off, rid, w, k, 1, out, out_off);
+}
+
+// bench: the sketch stage alone on device-resident packed reads, plain or homopolymer-compressed; *ms = CUDA-event time
+// of one call, the mean over `reps` calls after one untimed call (workspaces sized)
+extern "C" int wm_bench_sketch(const wm_bloom_s *bloom, int n, const char *seq, const int64_t *off, int w, int k, int is_hpc, int reps, double *ms)
+{
+	if (!(w > 0 && w < 256 && k > 0 && k <= 28) || n <= 0 || reps <= 0) return -1;
+	const int64_t tot = off[n];
+	char *d_ascii = wm_dev_alloc<char>(tot + 16);
+	uint32_t *d_pk = wm_dev_alloc<uint32_t>(wm_pk_words(tot)), *d_nm = wm_dev_alloc<uint32_t>(wm_nm_words(tot));
+	WM_CUDA_CHECK(cudaMemcpy(d_ascii, seq, tot, cudaMemcpyHostToDevice));
+	wm_pack_ascii(d_ascii, tot, d_pk, d_nm, 0);
+	wm_pkseq pks; pks.pk = d_pk, pks.nm = d_nm;
+	uint8_t *d_table = wm_dev_alloc<uint8_t>(bloom->table.size());
+	WM_CUDA_CHECK(cudaMemcpy(d_table, bloom->table.data(), bloom->table.size(), cudaMemcpyHostToDevice));
+	wm_bloom_dev bf; wm_bloom_dev_from_table(&bf, d_table, bloom->bits);
+	bf.n_salt = bloom->n_salt; bf.salt[0] = bloom->salt[0]; bf.salt[1] = bloom->salt[1];
+	std::vector<wm_sk_task> tasks(n);
+	for (int i = 0; i < n; ++i) tasks[i].seq_off = off[i], tasks[i].len = (int32_t)(off[i + 1] - off[i]), tasks[i].rid = 0;
+	wm_sketch_ws ws;
+	int64_t n_mz = 0;
+	cudaEvent_t e0, e1;
+	WM_CUDA_CHECK(cudaEventCreate(&e0)); WM_CUDA_CHECK(cudaEventCreate(&e1));
+	for (int r = -1; r < reps; ++r) {
+		if (r == 0) WM_CUDA_CHECK(cudaEventRecord(e0, 0));
+		if (is_hpc) wm_sketch_run_hpc(&ws, bf, pks, tasks.data(), n, w, k, &n_mz, 0);
+		else wm_sketch_run(&ws, bf, pks, tasks.data(), n, w, k, &n_mz, 0);
+	}
+	WM_CUDA_CHECK(cudaEventRecord(e1, 0));
+	WM_CUDA_CHECK(cudaEventSynchronize(e1));
+	float f = 0.f;
+	WM_CUDA_CHECK(cudaEventElapsedTime(&f, e0, e1));
+	*ms = f / reps;
+	cudaEventDestroy(e0); cudaEventDestroy(e1);
 	ws.release();
 	cudaFree(d_ascii); cudaFree(d_pk); cudaFree(d_nm); cudaFree(d_table);
 	return 0;

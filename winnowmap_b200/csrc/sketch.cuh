@@ -21,7 +21,12 @@ struct wm_sk_task {
 
 struct wm_sketch_ws {
 	wm_dbuf tasks, offs, ord, elig, flag, cnt, rank, scan_tmp, mz, mz_off;
-	void release() { tasks.release(); offs.release(); ord.release(); elig.release(); flag.release(); cnt.release(); rank.release(); scan_tmp.release(); mz.release(); mz_off.release(); }
+	wm_dbuf hpc_tasks, hpc_goff, hpc_coff, hpc_ends, hpc_pos, hpc_pk, hpc_nm; // the compressed pool of wm_sketch_run_hpc (untouched otherwise)
+	void release()
+	{
+		tasks.release(); offs.release(); ord.release(); elig.release(); flag.release(); cnt.release(); rank.release(); scan_tmp.release(); mz.release(); mz_off.release();
+		hpc_tasks.release(); hpc_goff.release(); hpc_coff.release(); hpc_ends.release(); hpc_pos.release(); hpc_pk.release(); hpc_nm.release();
+	}
 };
 
 struct wm_bloom_s;
@@ -33,5 +38,11 @@ void wm_pack_ascii(const char *d_in, int64_t n, uint32_t *d_pk, uint32_t *d_nm, 
 void wm_pack_gather(const char *d_pool, const int64_t *d_src_off, const int64_t *d_dst_off, int n_reads, int64_t n, uint32_t *d_pk, uint32_t *d_nm, cudaStream_t st);
 void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
                    int w, int k, int64_t *n_mz, cudaStream_t st);
+// the same on homopolymer-compressed sequences (mm_sketch with is_hpc = 1): the tasks are compacted on the device first;
+// positions and spans of the minimizers refer to the uncompressed bases
+void wm_sketch_run_hpc(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
+                       int w, int k, int64_t *n_mz, cudaStream_t st);
+// span (x & 0xff) of each of n minimizers
+void wm_mz_spans(const wm128_dev *d_mz, int64_t n, uint8_t *d_span, cudaStream_t st);
 void wm_bloom_dev_from_table(wm_bloom_dev *d, const uint8_t *d_table, uint64_t bits);
 void wm_bloom_params(const wm_bloom_s *b, uint64_t *bits, uint32_t *salt, int *n_salt);

@@ -122,8 +122,9 @@ class Bloom:
             pass
 
 
-def sketch_batch(bloom, seqs, w, k, rids=None):
-    """Batched mm_sketch (reference src/sketch.c:128).  seqs: list of bytes.  Returns list of (n,2) uint64."""
+def sketch_batch(bloom, seqs, w, k, rids=None, hpc=False):
+    """Batched mm_sketch (reference src/sketch.c:128).  seqs: list of bytes.  Returns list of (n,2) uint64.
+    hpc=True sketches homopolymer-compressed k-mers (is_hpc = 1)."""
     n = len(seqs)
     off = np.zeros(n + 1, dtype=np.int64)
     if n:
@@ -131,7 +132,8 @@ def sketch_batch(bloom, seqs, w, k, rids=None):
     buf = b"".join(seqs) + b"\0"
     rid = np.ascontiguousarray(rids if rids is not None else np.zeros(n), dtype=np.uint32)
     out, out_off = C.c_void_p(), C.c_void_p()
-    rc = lib().wm_sketch_batch(bloom.h, n, buf, _p(off, i64p), _p(rid, u32p), w, k, C.byref(out), C.byref(out_off))
+    fn = lib().wm_sketch_batch_hpc if hpc else lib().wm_sketch_batch
+    rc = fn(bloom.h, n, buf, _p(off, i64p), _p(rid, u32p), w, k, C.byref(out), C.byref(out_off))
     if rc != 0:
         raise ValueError("wm_sketch_batch failed")
     o = np.ctypeslib.as_array(C.cast(out_off, i64p), shape=(n + 1,)).copy()

@@ -29,6 +29,7 @@ class MapOpt(C.Structure):  # wm_mapopt_t == mm_mapopt_t (reference src/minimap.
 
 
 F_CIGAR, F_OUT_SAM, F_OUT_CG, F_NO_PRINT_2ND, F_PAF_NO_HIT = 0x004, 0x008, 0x020, 0x4000, 0x8000000
+I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
 
 STAT_NAMES = ("n_reads", "n_bases", "n_minimaps", "n_chained", "n_dp_jobs", "n_ll_jobs", "n_rounds", "t_seed", "t_dp", "t_host",
               "t_index", "t_map", "n_keys", "n_pos")
@@ -41,6 +42,9 @@ def _setup(L):
     L.wm_check_opt.argtypes = [C.POINTER(IdxOpt), C.POINTER(MapOpt)]
     L.wm_index_build.restype = C.c_void_p
     L.wm_index_build.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int]
+    L.wm_index_build_opt.restype = C.c_void_p
+    L.wm_index_build_opt.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(IdxOpt), C.c_int]
+    L.wm_idx_flag.argtypes = [C.c_void_p]
     L.wm_gpu_destroy.argtypes = [C.c_void_p]
     L.wm_idx_blob_size.restype = C.c_int64
     L.wm_idx_blob_size.argtypes = [C.c_void_p]
@@ -77,19 +81,27 @@ def make_options(preset=None, cigar=True, sam=False):
 
 
 class Mapper:
-    """winnowmap [-W rep.txt] -x preset -c ref.fa reads.fa  on one GPU."""
+    """winnowmap [-W rep.txt] -x preset [-H] -c ref.fa reads.fa  on one GPU.  hpc=True is -H: the index and the reads are
+    sketched with homopolymer-compressed k-mers (reference src/main.c:166).  A blob carries its own flag."""
 
-    def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False):
+    def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False):
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam)
+        if hpc:
+            self.io.flag |= I_HPC
         self.n_threads = n_threads or max(1, min(64, (os.cpu_count() or 2) // 2))
         if blob is not None:  # index received from another rank (numpy uint8 array)
             self._blob_keep = blob
             self.ctx = self.L.wm_idx_blob_load(blob.ctypes.data, blob.nbytes, device)
         else:
-            self.ctx = self.L.wm_index_build(ref.encode(), kmer_freq.encode() if kmer_freq else None, self.io.k, self.io.w, device)
+            self.ctx = self.L.wm_index_build_opt(ref.encode(), kmer_freq.encode() if kmer_freq else None, C.byref(self.io), device)
         if not self.ctx:
             raise RuntimeError("index construction failed")
+
+    @property
+    def hpc(self):
+        """True when the index holds homopolymer-compressed minimizers (MM_I_HPC)."""
+        return bool(self.L.wm_idx_flag(self.ctx) & I_HPC)
 
     def index_blob(self):
         """The flattened index as one numpy uint8 array (for the one-time NCCL fan-out)."""
