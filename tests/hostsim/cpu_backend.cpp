@@ -47,6 +47,7 @@ public:
 	// result storage
 	std::vector<std::vector<uint32_t>> mz_pos; std::vector<std::vector<uint64_t>> us; std::vector<std::vector<wm_pair_t>> bs;
 	std::vector<std::vector<uint32_t>> cigs;
+	std::vector<int64_t> n_anchors; // per task of the last seed_chain call: the anchors it chained (stage-1 and seeds)
 	void begin_batch(const std::vector<const wm_read*> &r) override { reads = r; }
 	void end_batch() override {}
 
@@ -54,7 +55,7 @@ public:
 	{
 		const int n = (int)tasks.size();
 		out.assign(n, SeedOut());
-		mz_pos.assign(n, {}); us.assign(n, {}); bs.assign(n, {});
+		mz_pos.assign(n, {}); us.assign(n, {}); bs.assign(n, {}); n_anchors.assign(n, 0);
 		#pragma omp parallel for schedule(dynamic, 4)
 		for (int i = 0; i < n; ++i) {
 			const SeedTask &t = tasks[i];
@@ -95,6 +96,7 @@ public:
 				if (!a.empty()) wmo_radix_sort_128x(w.data(), (long)w.size());
 				a.swap(w);
 			}
+			n_anchors[i] = (int64_t)a.size();
 			const ChainParams &c = cp[t.chain_set];
 			us[i].resize(a.size() + 1); bs[i].resize(a.size() + 1);
 			long nb = 0;
@@ -157,9 +159,9 @@ public:
 static int g_gap_override[4] = {0, 0, 0, 0}; // -O / -E of the next run (0 = keep the preset's)
 extern "C" void wmt_set_gap(int q, int e, int q2, int e2) { g_gap_override[0] = q, g_gap_override[1] = e, g_gap_override[2] = q2, g_gap_override[3] = e2; }
 
-static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *preset, const char *reads_fn, const char *out_fn, int n_threads, int sam, int64_t extra_flags = 0)
+// the options of one run: preset, -c or -a, extra output flags and the one-shot -O / -E override
+static int run_opts(const char *preset, int sam, int64_t extra_flags, wm_idxopt_t &io, wm_mapopt_t &mo)
 {
-	wm_idxopt_t io; wm_mapopt_t mo;
 	set_opt(0, &io, &mo);
 	if (preset && set_opt(preset, &io, &mo) < 0) return -1;
 	if (sam) mo.flag |= WM_F_OUT_SAM | WM_F_CIGAR; // -a (src/main.c)
@@ -167,31 +169,46 @@ static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *pr
 	mo.flag |= extra_flags;                        // --cs / --cs=long / --MD (src/main.c:227,249-266)
 	if (g_gap_override[0] > 0) mo.q = g_gap_override[0], mo.e = g_gap_override[1], mo.q2 = g_gap_override[2], mo.e2 = g_gap_override[3]; // -O / -E (src/main.c)
 	g_gap_override[0] = 0; // one shot
-	if (check_opt(&io, &mo) < 0) return -2;
-	wm_host_idx H; H.k = io.k, H.w = io.w;
-	std::vector<uint64_t> kmers;
-	if (read_kmer_list(kmer_fn, io.k, kmers) < 0) return -3;
-	void *bloom = wmo_bloom_init(kmers.size());
-	for (uint64_t k : kmers) wmo_bloom_insert(bloom, k);
-	std::vector<uint64_t> mz;
-	{
-		SeqReader rd;
-		if (!rd.open(ref_fn)) return -4;
-		wm_read r; uint64_t sum_len = 0;
-		while (rd.next(r)) {
-			const uint32_t rid = (uint32_t)H.name.size();
-			H.name.push_back(r.name); H.len.push_back((uint32_t)r.seq.size()); H.offset.push_back(sum_len);
-			H.S.resize((sum_len + r.seq.size() + 7) / 8, 0);
-			for (size_t j = 0; j < r.seq.size(); ++j) { uint64_t o = sum_len + j; uint8_t c = code_of(r.seq[j]); if (r.seq[j] == 'U' || r.seq[j] == 'u') c = 4; H.S[o >> 3] |= (uint32_t)c << ((o & 7) << 2); }
-			sum_len += r.seq.size();
-			if (r.seq.empty()) continue;
-			std::vector<uint64_t> tmp((size_t)2 * (r.seq.size() / 2 + 64));
-			long n = wmo_sketch(r.seq.data(), (int)r.seq.size(), io.w, io.k, rid, bloom, tmp.data(), (long)tmp.size() / 2);
-			mz.insert(mz.end(), tmp.begin(), tmp.begin() + 2 * n);
-		}
+	return check_opt(&io, &mo) < 0 ? -2 : 0;
+}
+
+// The host index of a reference: names, lengths, 4-bit packed bases, the down-weight filter of the k-mer list and the
+// oracle's minimizers of every sequence (in position order, as wmo_sketch emits them).
+struct OracleIndex {
+	wm_host_idx H;
+	std::vector<uint64_t> kmers; // the -W list, canonical k-mers
+	std::vector<uint64_t> mz;    // x, y pairs
+	void *bloom = 0;
+	~OracleIndex() { if (bloom) wmo_bloom_free(bloom); }
+};
+
+static int load_oracle_index(const char *ref_fn, const char *kmer_fn, int k, int w, OracleIndex &X)
+{
+	wm_host_idx &H = X.H;
+	H.k = k, H.w = w;
+	if (read_kmer_list(kmer_fn, k, X.kmers) < 0) return -3;
+	X.bloom = wmo_bloom_init(X.kmers.size());
+	for (uint64_t km : X.kmers) wmo_bloom_insert(X.bloom, km);
+	SeqReader rd;
+	if (!rd.open(ref_fn)) return -4;
+	wm_read r; uint64_t sum_len = 0;
+	while (rd.next(r)) {
+		const uint32_t rid = (uint32_t)H.name.size();
+		H.name.push_back(r.name); H.len.push_back((uint32_t)r.seq.size()); H.offset.push_back(sum_len);
+		H.S.resize((sum_len + r.seq.size() + 7) / 8, 0);
+		for (size_t j = 0; j < r.seq.size(); ++j) { uint64_t o = sum_len + j; uint8_t c = code_of(r.seq[j]); if (r.seq[j] == 'U' || r.seq[j] == 'u') c = 4; H.S[o >> 3] |= (uint32_t)c << ((o & 7) << 2); }
+		sum_len += r.seq.size();
+		if (r.seq.empty()) continue;
+		std::vector<uint64_t> tmp((size_t)2 * (r.seq.size() / 2 + 64));
+		long n = wmo_sketch(r.seq.data(), (int)r.seq.size(), w, k, rid, X.bloom, tmp.data(), (long)tmp.size() / 2);
+		X.mz.insert(X.mz.end(), tmp.begin(), tmp.begin() + 2 * n);
 	}
-	CpuBackend be;
-	be.hidx = &H; be.bloom = bloom; be.idx = wmo_idx_build(mz.data(), (long)mz.size() / 2);
+	return 0;
+}
+
+// Maps every read of `reads_fn` through `be` (one batch, longest reads first) and writes PAF or SAM to `out_fn`.
+static int map_reads_to(Backend *be, const wm_host_idx &H, const wm_mapopt_t &mo, const char *reads_fn, const char *out_fn, int n_threads, int sam)
+{
 	SeqReader rd;
 	if (!rd.open(reads_fn)) return -5;
 	std::vector<wm_read> batch; wm_read r;
@@ -202,7 +219,7 @@ static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *pr
 	std::vector<const wm_read*> reads;
 	for (auto &o : ord) reads.push_back(&batch[o.second]);
 	std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-	map_batch(&be, &H, &mo, reads, regs, rl, fg, n_threads, 0);
+	map_batch(be, &H, &mo, reads, regs, rl, fg, n_threads, 0);
 	FILE *out = fopen(out_fn, "wb");
 	std::string line;
 	int n_gen_mismatch = 0;
@@ -229,8 +246,21 @@ static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *pr
 		for (auto &rr : regs[i]) free(rr.p);
 	}
 	fclose(out);
-	wmo_idx_free(be.idx); wmo_bloom_free(bloom);
 	return n_gen_mismatch ? -100 - n_gen_mismatch : 0;
+}
+
+static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *preset, const char *reads_fn, const char *out_fn, int n_threads, int sam, int64_t extra_flags = 0)
+{
+	wm_idxopt_t io; wm_mapopt_t mo;
+	int rc = run_opts(preset, sam, extra_flags, io, mo);
+	if (rc < 0) return rc;
+	OracleIndex X;
+	if ((rc = load_oracle_index(ref_fn, kmer_fn, io.k, io.w, X)) < 0) return rc;
+	CpuBackend be;
+	be.hidx = &X.H; be.bloom = X.bloom; be.idx = wmo_idx_build(X.mz.data(), (long)X.mz.size() / 2);
+	rc = map_reads_to(&be, X.H, mo, reads_fn, out_fn, n_threads, sam);
+	wmo_idx_free(be.idx);
+	return rc;
 }
 
 // winnowmap [-W kmers] -x preset -c ref.fa reads.fa > out.paf, host orchestration on the oracle backend

@@ -279,7 +279,7 @@ class OracleBloom:
 
 
 def oracle_sketch(seq: bytes, w, k, rid, bloom: OracleBloom):
-    cap = len(seq) // 4 + 64
+    cap = len(seq) + 64  # w = 1: up to one minimizer per base
     out = np.zeros(cap * 2, dtype=np.uint64)
     n = oracle().wmo_sketch(seq, len(seq), w, k, rid, bloom.h if bloom else None, _ptr(out, _u64p), cap)
     assert n <= cap
@@ -304,7 +304,7 @@ class RefSketch:
         return bool(self.L.ref_bloom_contains(self.h, int(k)))
 
     def sketch(self, seq: bytes, w, k, rid):
-        cap = len(seq) // 4 + 64
+        cap = len(seq) + 64  # w = 1: up to one minimizer per base
         out = np.zeros(cap * 2, dtype=np.uint64)
         n = self.L.ref_sketch(self.h, seq, len(seq), w, k, rid, _ptr(out, _u64p), cap)
         assert n <= cap

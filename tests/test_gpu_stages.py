@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
-from test_oracle_vs_ref import make_anchors
+from test_oracle_vs_ref import make_anchors, make_span_anchors
 
 pytestmark = pytest.mark.gpu
 TESTS_DIR = os.path.dirname(os.path.abspath(__file__))
@@ -35,10 +35,13 @@ def _seq_set(rng, kmers, k):
         seqs.append(bytes(planted))
     # many windows of one read, as in stage 1
     seqs += [base[i:i + 2000] for i in range(0, 20000, 2000)]
+    seqs += [base[:1023], base[1:1025], base[2:1027]]  # around the 1024-base sketch tile
     return seqs
 
 
-@pytest.mark.parametrize("n_k,k,w", [(0, 15, 50), (255, 15, 50), (5000, 15, 50), (300, 19, 50), (255, 15, 10), (0, 16, 20), (0, 6, 20)])
+# k = 27 / 28: the largest k of the parallel order kernel and of the sequential one, at the smallest and largest w
+@pytest.mark.parametrize("n_k,k,w", [(0, 15, 50), (255, 15, 50), (5000, 15, 50), (300, 19, 50), (255, 15, 10), (0, 16, 20), (0, 6, 20),
+                                     (0, 27, 1), (255, 27, 255), (0, 28, 1), (255, 28, 255)])
 def test_sketch_matches_oracle(n_k, k, w):
     from winnowmap_b200 import kernels
     rng = np.random.default_rng(1000 + n_k + k + w)
@@ -100,6 +103,7 @@ def test_chain_matches_oracle(seed):
     from winnowmap_b200 import kernels
     rng = np.random.default_rng(500 + seed)
     arrays = [make_anchors(rng, n, repeats=bool((seed + i) & 1)) for i, n in enumerate([0, 1, 3, 10, 40, 100, 100, 700, 3000, 9000] * 3)]
+    arrays += [make_span_anchors(rng, n, repeats=bool((seed + i) & 1)) for i, n in enumerate([1, 10, 100, 700, 3000, 9000])]
     for prm in [dict(max_dist_x=5000, min_dist_x=1000, max_dist_y=5000, bw=500), dict(max_dist_x=16000, min_dist_x=1000, max_dist_y=16000, bw=2000),
                 dict(max_dist_x=5000, min_dist_x=50, max_dist_y=5000, bw=500, max_iter=20, max_skip=3)]:
         got = kernels.chain_dp_batch(arrays, **prm)
@@ -122,6 +126,15 @@ def _tandem_anchors(rng, n_q, n_copies, unit, span=15):
     return ol.ref_sort128(xy) if ol.have_ref() else ol.oracle_sort128(xy)
 
 
+def _span_tandem(rng):
+    """A tandem lattice whose anchors carry spans from 1 to 255 and, on some, the tandem flag (bit 42 of y)."""
+    a = _tandem_anchors(rng, 150, 60, 171)
+    span = rng.integers(1, 256, size=len(a)).astype(np.uint64)
+    tandem = (rng.random(len(a)) < 0.3).astype(np.uint64) << np.uint64(42)
+    a[:, 1] = (a[:, 1] & np.uint64(0xffffffff)) | span << np.uint64(32) | tandem
+    return ol.oracle_sort128(a)  # ties in x are ordered by y, flags included
+
+
 @pytest.mark.parametrize("tile_min", [None, 1])
 def test_chain_giant_tasks_match_oracle(tile_min, tmp_path):
     """Giant tasks go through the tile kernel (one CTA per task, one warp per anchor of a 32-anchor tile, csrc/chain.cu): tandem
@@ -135,11 +148,12 @@ sys.path.insert(0, %r); sys.path.insert(0, %r)
 import numpy as np
 import oracle_lib as ol
 from winnowmap_b200 import kernels
-from test_oracle_vs_ref import make_anchors
-from test_gpu_stages import _tandem_anchors
+from test_oracle_vs_ref import make_anchors, make_span_anchors
+from test_gpu_stages import _tandem_anchors, _span_tandem
 rng = np.random.default_rng(78)
 arrays = [_tandem_anchors(rng, 120, 100, 171), _tandem_anchors(rng, 300, 200, 340), _tandem_anchors(rng, 60, 40, 64), make_anchors(rng, 9000, repeats=True),
-          make_anchors(rng, 5000, repeats=False), make_anchors(rng, 33, repeats=True), make_anchors(rng, 1, repeats=False)]
+          make_anchors(rng, 5000, repeats=False), make_anchors(rng, 33, repeats=True), make_anchors(rng, 1, repeats=False),
+          make_span_anchors(rng, 9000, repeats=True), make_span_anchors(rng, 5000, repeats=False), _span_tandem(rng)]
 for prm in [dict(max_dist_x=5000, min_dist_x=1000, max_dist_y=5000, bw=500), dict(max_dist_x=16000, min_dist_x=1000, max_dist_y=16000, bw=2000),
             dict(max_dist_x=5000, min_dist_x=50, max_dist_y=5000, bw=500, max_iter=20, max_skip=3)]:
     got = kernels.chain_dp_batch(arrays, **prm)

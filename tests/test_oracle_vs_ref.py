@@ -207,6 +207,19 @@ def test_bloom_and_sketch_match_reference():
         for w in (50, 10):
             for si, sq in enumerate(seqs):
                 ol.assert_ref(f"sketch:{n_k}:{k}:{w}:{si}", ol.oracle_sketch(sq, w, k, 3, ob), lambda: rb.sketch(sq, w, k, 3))
+    # the largest k of the parallel (27) and of the sequential (28) device kernel at the smallest and largest w; lengths
+    # around the 1024-base sketch tile
+    for n_k, k in [(0, 27), (300, 27), (0, 28), (300, 28)]:
+        kmers = rng.integers(0, 1 << (2 * k), size=n_k, dtype=np.uint64)
+        ob, rb = ol.OracleBloom(kmers), ol.RefSketch(kmers) if ol.recording() else None
+        base = bytes(b"ACGT"[c] for c in rng.integers(0, 4, size=12000, dtype=np.uint8))
+        s2 = bytearray(base[:5000])
+        for p in range(300, 4500, 700):
+            s2[p:p + int(rng.integers(1, 60))] = b"N" * 60
+        seqs = [base, base[:1023], base[1:1025], base[2:1027], bytes(s2), base[:27] + b"N" + base[27:100]]
+        for w in (1, 255):
+            for si, sq in enumerate(seqs):
+                ol.assert_ref(f"sketch_edge:{n_k}:{k}:{w}:{si}", ol.oracle_sketch(sq, w, k, 3, ob), lambda: rb.sketch(sq, w, k, 3))
 
 
 def test_sketch_even_k_symmetric_kmers():
@@ -232,13 +245,31 @@ def make_anchors(rng, n, span=15, repeats=False):
     return ol.oracle_sort128(xy)
 
 
+def make_span_anchors(rng, n, repeats=False):
+    """Anchors with the spans of homopolymer-compressed minimizers (1 to 255, so that the average span the gap cost uses is
+    not an integer) and the tandem flag (bit 42 of y) on some of them."""
+    a = make_anchors(rng, n, repeats=repeats)
+    if n:
+        span = rng.integers(1, 256, size=n).astype(np.uint64)
+        tandem = (rng.random(n) < 0.2).astype(np.uint64) << np.uint64(42)
+        a[:, 1] = (a[:, 1] & np.uint64(0xffffffff)) | span << np.uint64(32) | tandem
+        a = ol.oracle_sort128(a)  # ties in x are ordered by y, flags included
+    return a
+
+
 @pytest.mark.parametrize("seed", range(4))
 def test_chain_matches_reference(seed):
     rng = np.random.default_rng(400 + seed)
+    rs = np.random.default_rng(450 + seed)  # the varying-span inputs draw from their own stream
     for n in [0, 1, 3, 10, 100, 700, 3000]:
         a = make_anchors(rng, n, repeats=bool(seed & 1))
         for (mx, mn, my, bw) in [(5000, 1000, 5000, 500), (16000, 1000, 16000, 2000)]:
             ol.assert_ref(f"chain:{seed}:{n}:{mx}", ol.oracle_chain(a, mx, mn, my, bw), lambda: ol.ref_chain(a, mx, mn, my, bw))
         # small max_iter exercises the Winnowmap window rule (chain.c:52-55)
         ol.assert_ref(f"chain_window:{seed}:{n}", ol.oracle_chain(a, 5000, 50, 5000, 500, max_iter=20, max_skip=3),
+                      lambda: ol.ref_chain(a, 5000, 50, 5000, 500, max_iter=20, max_skip=3))
+        a = make_span_anchors(rs, n, repeats=bool(seed & 1))
+        for (mx, mn, my, bw) in [(5000, 1000, 5000, 500), (16000, 1000, 16000, 2000)]:
+            ol.assert_ref(f"chain_span:{seed}:{n}:{mx}", ol.oracle_chain(a, mx, mn, my, bw), lambda: ol.ref_chain(a, mx, mn, my, bw))
+        ol.assert_ref(f"chain_span_window:{seed}:{n}", ol.oracle_chain(a, 5000, 50, 5000, 500, max_iter=20, max_skip=3),
                       lambda: ol.ref_chain(a, 5000, 50, 5000, 500, max_iter=20, max_skip=3))
