@@ -125,6 +125,21 @@ public:
 		const int n = (int)tasks.size();
 		bool set_used[2] = {false, false};
 		add("seed.calls"); add("seed.tasks", n);
+		// tasks of this call per worker class of the CTA kernels, as peaks over calls: above 1, some worker of a class whose
+		// grid is capped at one CTA (WM_SORT_MEDIUM_CTAS / WM_SORT_GIANT_CTAS / WM_CHAIN_TILE_CTAS = 1) took a second task
+		const int64_t tile_min = env_int("WM_CHAIN_TILE_MIN", 2048), bt_cta_min = env_int("WM_CHAIN_BT_CTA_MIN", 4096);
+		const int64_t giant_min = env_int("WM_SORT_GIANT_MIN", 0) >= 2048 ? env_int("WM_SORT_GIANT_MIN", 0) : 1 << 30; // seed.cu
+		int64_t n_tile = 0, n_bt_cta = 0, n_sort_medium[3] = {0, 0, 0}, n_sort_giant[3] = {0, 0, 0};
+		for (int i = 0; i < n; ++i) { // sort launches (gpu_backend.cu seed_chain): the seeds of the plain and of the masked pass, then sort #3
+			const SeedTask &t = tasks[i];
+			const int64_t n_a = fetcher->n_anchors[i], n_seed = n_a - t.n_pre;
+			const int64_t sz[3] = {(t.flags & (SEED_MASKED | SEED_NO_SKETCH)) ? 0 : n_seed, (t.flags & SEED_MASKED) ? n_seed : 0,
+			                       t.n_pre > 0 && n_seed > 0 ? n_a : 0};
+			for (int l = 0; l < 3; ++l) { n_sort_medium[l] += sz[l] > 2048 && sz[l] <= giant_min; n_sort_giant[l] += sz[l] > giant_min; }
+			n_tile += n_a > tile_min; n_bt_cta += n_a > bt_cta_min;
+		}
+		peak("peak.chain_tile", n_tile); peak("peak.chain_bt_cta", n_bt_cta);
+		for (int l = 0; l < 3; ++l) { peak("peak.sort_medium", n_sort_medium[l]); peak("peak.sort_giant", n_sort_giant[l]); }
 		for (int i = 0; i < n; ++i) {
 			const SeedTask &t = tasks[i];
 			const SeedOut &e = eo[i], &g = out[i];
@@ -193,7 +208,9 @@ public:
 			if (nc > 0) cmp_arr("run_dp", call, i, "cigar", e.cigar, g.cigar, nc, [](uint32_t c) { return dec(c >> 4) + "MIDN"[c & 3]; }, desc);
 			if (!(J.flag & EZ_SCAN_ZDROP)) continue;
 			add("dp.scan_zdrop_jobs");
-			if (J.q.len <= 0 || J.t.len <= 0) continue; // nothing aligned: no walk
+			// nothing aligned (an empty input, or a scoring the reference returns on before the sweep): no walk on the device,
+			// host_align.cpp walks the empty CIGAR itself
+			if (J.q.len <= 0 || J.t.len <= 0 || (e.n_cigar == 0 && !g.has_zd)) continue;
 			if (!g.has_zd) { bad("run_dp", call, i, "has_zd", -1, "1", dec(g.has_zd), desc); continue; }
 			std::vector<uint8_t> qs, ts;
 			fetcher->fetch(J.q, wins[J.task], qs); fetcher->fetch(J.t, wins[J.task], ts);

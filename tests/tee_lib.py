@@ -353,10 +353,12 @@ def crafted_ll_jobs(wins, contigs, rng, n=60):
     return rows
 
 
-SCORINGS = {  # (match, mismatch, q, e, q2, e2): map-ont, asm20-like, and one gap pair (ksw_extz2)
+SCORINGS = {  # (match, mismatch, q, e, q2, e2): map-ont, asm20-like, one gap pair (ksw_extz2), and a mismatch above 2(q + e),
+    # for which ksw_extd2_sse returns before the sweep (src/ksw2_extd2_sse.c:92; -B13 with map-ont's gaps)
     "map-ont": (2, 4, 4, 2, 24, 1),
     "asm20": (1, 4, 6, 2, 26, 1),
     "single": (2, 4, 4, 2, 4, 2),
+    "early-out": (1, 13, 4, 2, 24, 1),
 }
 
 

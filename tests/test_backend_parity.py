@@ -120,6 +120,41 @@ def test_whole_path_matches_oracle_under_tuning_switches(tee_so, tmp_path):
     assert r["chain.bt_cta_tasks"] > r["chain.gt4096"], r.text()
 
 
+# One CTA for the medium sort, the giant sort and the chaining tile kernel, with low thresholds for the giant classes: a
+# worker that takes two tasks carries its state (mbarrier phases, work lists, rings, masks) from the first into the second.
+TASK_LOOP_ENV = {"WM_SORT_MEDIUM_CTAS": "1", "WM_SORT_GIANT_MIN": "4096", "WM_SORT_GIANT_CTAS": "1", "WM_CHAIN_TILE_MIN": "256",
+                 "WM_CHAIN_TILE_CTAS": "1", "WM_CHAIN_BT_CTA_MIN": "256"}
+# The classes (tasks of one launch, peak over launches) each run reaches more than once under TASK_LOOP_ENV.  No run has two
+# arrays of 2049-4096 anchors in one sort launch, so the medium sort's second array is left to tests/test_gpu_task_loops.py.
+TASK_LOOP_PEAKS = {
+    "ont_highocc": ["peak.chain_tile", "peak.chain_bt_cta", "peak.sort_giant"],
+    "ont_tandem": ["peak.chain_tile", "peak.chain_bt_cta"],  # no anchor array above 2048
+    "hpc_ont_small": [],  # at most one task above 256 anchors per call, no array above 2048: zero mismatches and the golden only
+    "seed": ["peak.chain_tile", "peak.chain_bt_cta", "peak.sort_giant"],
+    "seed_hpc": ["peak.chain_tile", "peak.chain_bt_cta", "peak.sort_giant"],
+}
+
+
+@pytest.mark.parametrize("name", ["ont_highocc", "ont_tandem", "hpc_ont_small"])
+def test_whole_path_task_loops_match_oracle(tee_so, name, tmp_path):
+    """Whole mapping runs with single-CTA grids for the sorts and the tile kernel: zero mismatches, the golden output, and
+    some worker of each forced class took a second task."""
+    case = _map_case(name, tmp_path)
+    r = _run(tee_so, case, tmp_path, env=TASK_LOOP_ENV)
+    _check_map(r, case)
+    for key in TASK_LOOP_PEAKS[name]:
+        assert r[key] > 1, (key, r.text())
+
+
+@pytest.mark.parametrize("hpc", [False, True])
+def test_crafted_seed_chain_task_loops_match_oracle(tee_so, hpc, tmp_path):
+    """The crafted stage-1 / stage-2 seed batches of test_crafted_seed_chain_matches_oracle under the same single-CTA grids."""
+    r = _run(tee_so, dict(kind="seed", ref=str(tmp_path / "ref.fa"), k=15, w=10, hpc=int(hpc)), tmp_path, env=TASK_LOOP_ENV)
+    assert r.n_mismatch == 0, r.text()
+    for key in TASK_LOOP_PEAKS["seed_hpc" if hpc else "seed"]:
+        assert r[key] > 1, (key, r.text())
+
+
 @pytest.mark.parametrize("hpc", [False, True])
 def test_crafted_seed_chain_matches_oracle(tee_so, hpc, tmp_path):
     """A stage-1 call: windows at odd starts and at the read end, lengths around k, w + k - 1, 128 and 1024 and tens of kb;

@@ -147,6 +147,20 @@ def test_extd2_swapped_gap_and_asm_scoring():
             ol.assert_ref(f"extd2_swapped:{a},{b},{q},{e},{q2},{e2}:{it}", got, lambda: ol.ref_extd2(qq, tt, mat, q, e, q2, e2, 200, 200, -1, flag))
 
 
+def test_early_out_scoring_matches_reference():
+    """A mismatch score above 2(q + e) (-B13 with map-ont's -O4 -E2): ksw_extd2_sse and ksw_extz2_sse return before the sweep
+    (src/ksw2_extd2_sse.c:92, src/ksw2_extz2_sse.c:82), leaving the initial ksw_extz_t and no CIGAR, whatever the inputs."""
+    rng = np.random.default_rng(13)
+    mat = ol.simple_mat(1, 13)
+    for it in range(12):
+        qq, tt = rand_pair(rng, int(rng.choice([1, 40, 600, 2500])), err=0.05, drift=int(rng.choice([0, 50])))
+        w, flag = [3001, 751, 50, -1][it % 4], FLAGS[it % 4] | (0x10 if it % 3 == 0 else 0)
+        got = ol.oracle_extd2(qq, tt, mat, 4, 2, 24, 1, w, 400, -1, flag)
+        ol.assert_ref(f"extd2_early_out:{it}", got, lambda: ol.ref_extd2(qq, tt, mat, 4, 2, 24, 1, w, 400, -1, flag))
+        got = ol.oracle_extz2(qq, tt, mat, 4, 2, w, 400, -1, flag)
+        ol.assert_ref(f"extz2_early_out:{it}", got, lambda: ol.ref_extz2(qq, tt, mat, 4, 2, w, 400, -1, flag))
+
+
 @pytest.mark.parametrize("seed", range(3))
 def test_ll_matches_reference(seed):
     rng = np.random.default_rng(300 + seed)

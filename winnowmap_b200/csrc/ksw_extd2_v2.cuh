@@ -341,6 +341,9 @@ __device__ void wm_extd2_fill_job_v2_cta(const wm_dp_job &J, const uint8_t *__re
 	ez.max_q = ez.max_t = ez.mqe_t = ez.mte_q = -1;
 	ez.max = 0, ez.score = ez.mqe = ez.mte = WM_NEG_INF;
 	ez.n_cigar = 0, ez.zdropped = 0, ez.reach_end = 0, ez.reserved = 0;
+	// a mismatch score above 2(q+e) makes the reference return before the sweep (src/ksw2_extd2_sse.c:92), as the warp
+	// kernel does (wm_extd2_fill_job); P is uniform, so the whole CTA returns here
+	if (P.early_out) { if (tid == 0) *out = ez; return; }
 	const int q = P.q, e = P.e, q2 = P.q2, e2 = P.e2;
 	const bool approx_max = (flag & 0x08) != 0, right = (flag & 0x02) != 0;
 	if (w < 0) w = tlen > qlen ? tlen : qlen;
