@@ -259,13 +259,18 @@ wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
 
 /* Replaces kt_for(p->n_threads, worker_for, in, n_frag) (src/map.c:1162-1165; worker_for :1008-1048): one call per
  * mini-batch, blocking; fills n_reg[i], reg[i] (malloc()ed array whose ->p are malloc()ed, freed by the caller as
- * at src/map.c:1210-1211), rep_len[i] and frag_gap[i] (src/map.c:1025-1034).  n_threads = host threads for the glue. */
+ * at src/map.c:1210-1211), rep_len[i] and frag_gap[i] (src/map.c:1025-1034).  n_threads = host threads for the glue.
+ * opt->flag may carry MM_F_NO_DIAG (-D), MM_F_NO_DUAL (--dual=no), both with MM_F_ALL_CHAINS | MM_F_NO_LJOIN (-X), and
+ * MM_F_FOR_ONLY / MM_F_REV_ONLY (--for-only / --rev-only): the seed filter of skip_seed (src/map.c:132-154) runs on the
+ * device.  Its name tests compare names[i] with the index's sequence names; names == NULL or names[i] == NULL is a read
+ * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE, MM_F_SR and MM_F_HEAP_SORT are refused. */
 int wm_gpu_map_batch(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, int n_seq, const char *const *names, const char *const *seqs,
                      const int32_t *lens, int32_t *n_reg, wm_reg1_t **reg, int32_t *rep_len, int32_t *frag_gap, int n_threads);
 
 /* mm_tbuf_init / mm_tbuf_destroy / mm_map (src/minimap.h:329-351, src/map.c:18-38, :976-984): one read through the same path
  * (internally a batch of one).  The returned array and every ->p are malloc()ed and freed by the caller, as with mm_map.
- * The buffer carries what mm_tbuf_s carries for the caller: rep_len and frag_gap of the last call. */
+ * The buffer carries what mm_tbuf_s carries for the caller: rep_len and frag_gap of the last call.  name == NULL is mm_map
+ * with qname == 0: under -D / --dual=no / -X the name tests of the seed filter are off (an empty name "" is a name). */
 typedef struct wm_tbuf_s wm_tbuf_t;
 wm_tbuf_t *wm_tbuf_init(void);
 void wm_tbuf_destroy(wm_tbuf_t *b);
@@ -276,7 +281,9 @@ wm_reg1_t *wm_map(wm_gpu_ctx *ctx, int l_seq, const char *seq, int *n_regs, wm_t
 /* mm_map_file (src/map.c:1273) into out_fn ("-" = stdout): PAF (mm_write_paf3, src/format.c:308), or SAM when
  * opt->flag has MM_F_OUT_SAM (mm_write_sam3, src/format.c:391, single-segment reads; header as mm_write_sam_hdr,
  * src/format.c:118, written by rank 0 when tag_order == 0).  rank/world shard the reads of every mini-batch
- * round-robin over processes (one process per GPU); tag_order prefixes "<batch>\t<pos>\t" for merging. */
+ * round-robin over processes (one process per GPU); tag_order prefixes "<batch>\t<pos>\t" for merging.  Accepts the
+ * flags wm_gpu_map_batch accepts: -X reads.fa against an index of reads.fa computes read overlaps, -D asm.fa against
+ * asm.fa self-alignments; the filter depends only on the read and the index, so sharding needs nothing more. */
 int wm_map_file(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, int n_threads, int rank, int world,
                 int tag_order, int64_t max_batch_bases);
 /* the command line recorded in the @PG header line of SAM output (the reference prints its own argv, src/format.c:130-135) */

@@ -390,8 +390,72 @@ def main_hpc():
     json.dump(manifest, open(os.path.join(gdir, "hpc_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- self and all-vs-all mapping (-X, -D, --dual=no) and single-strand mapping (--for-only, --rev-only) ----
+# tests/golden/overlap_manifest.json and overlap_*.paf.gz; the other manifests are not touched.
+# Inputs: "ava" maps a read set against itself (reads of 2-40 kb: both the stage-1 route, reads >= 10 kb, and the
+# whole-read route); "asm" maps the reads of hifi_small against themselves; "tandem" is the ont_tandem case.
+AVA = dict(ref_len=200000, contigs=1, ref_seed=7, n_reads=80, n50=12000, err=0.05, read_seed=8, min_len=2000)
+OVERLAP_CASES = {
+    # name: (inputs, reference options, library options of Mapper)
+    "overlap_ava_X": ("ava", ["-x", "map-ont", "-X"], dict(preset="map-ont", cigar=False, all_vs_all=True)),
+    "overlap_ava_X_c": ("ava", ["-x", "map-ont", "-X", "-c"], dict(preset="map-ont", all_vs_all=True)),
+    "overlap_ava_D_c": ("ava", ["-x", "map-ont", "-D", "-c"], dict(preset="map-ont", no_diag=True)),
+    "overlap_asm_D_c": ("asm", ["-x", "asm20", "-D", "-c"], dict(preset="asm20", no_diag=True)),
+    "overlap_ava_dual_no": ("ava", ["-x", "map-ont", "--dual=no", "-c"], dict(preset="map-ont", dual=False)),
+    "overlap_tandem_for_only": ("tandem", ["-x", "map-ont", "--for-only", "-c"], dict(preset="map-ont", strand="for")),
+    "overlap_tandem_rev_only": ("tandem", ["-x", "map-ont", "--rev-only", "-c"], dict(preset="map-ont", strand="rev")),
+    "overlap_ava_X_H": ("ava", ["-x", "map-ont", "-X", "-H"], dict(preset="map-ont", cigar=False, all_vs_all=True, hpc=True)),
+    "overlap_ava_X_sam": ("ava", ["-x", "map-ont", "-X", "-a"], dict(preset="map-ont", sam=True, all_vs_all=True)),
+}
+
+
+def make_overlap_inputs(inputs, outdir):
+    """(index FASTA, reads FASTA, -W file or None) of one overlap input set."""
+    if inputs == "ava":
+        os.makedirs(outdir, exist_ok=True)
+        c = AVA
+        genome = gen_data.make_ref(np.random.default_rng(c["ref_seed"]), c["ref_len"], c["contigs"], False)
+        reads = os.path.join(outdir, "overlap_ava.reads.fa")
+        recs = gen_data.make_reads(np.random.default_rng(c["read_seed"]), genome, c["n_reads"], c["n50"], c["err"], min_len=c["min_len"])
+        gen_data.write_fasta(reads, recs)
+        return reads, reads, None
+    if inputs == "asm":  # low-error sequences of 1-40 kb from a genome with tandem arrays, as contigs
+        _, reads, _ = make_inputs("hifi_small", outdir)
+        return reads, reads, None
+    return make_inputs("ont_tandem", outdir)
+
+
+def main_overlap():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_overlap"
+    manifest = {}
+    for name, (inputs, args, lib_opts) in OVERLAP_CASES.items():
+        ref, reads, wfile = make_overlap_inputs(inputs, tmp)
+        cmd = [refbin, "-t", "4"] + args + (["-W", wfile] if wfile else []) + [ref, reads]
+        out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+        m = dict(inputs=inputs, lib=lib_opts, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile) if wfile else None,
+                 cmd=" ".join(["winnowmap"] + cmd[1:]))
+        if lib_opts.get("sam"):
+            body = sam_without_pg(out)
+            with gzip.GzipFile(os.path.join(gdir, name + ".sam.stripped.gz"), "wb", mtime=0) as f:
+                f.write(sam_strip_seq(body))
+            m["sam_md5"], m["n_lines"] = hashlib.md5(body).hexdigest(), body.count(b"\n")
+        else:
+            with gzip.GzipFile(os.path.join(gdir, name + ".paf.gz"), "wb", mtime=0) as f:
+                f.write(out)
+            m["paf_md5"], m["n_lines"] = hashlib.md5(out).hexdigest(), out.count(b"\n")
+        manifest[name] = m
+        print(name, m["n_lines"], "lines")
+    json.dump(manifest, open(os.path.join(gdir, "overlap_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
     if "--hpc" in sys.argv:
         main_hpc()
+    elif "--overlap" in sys.argv:
+        main_overlap()
     else:
         main()

@@ -179,6 +179,7 @@ extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload_flag(const wm_idx_view_t *v, int idx_
 		c->hidx.offset.push_back(v->seq_offset[i]);
 	}
 	c->hidx.S.assign(v->S, v->S + v->S_words);
+	set_name_order(&c->hidx);
 	c->n_keys = v->n_keys, c->n_pos = (int64_t)v->pos_off[v->n_keys];
 	c->keys.assign(v->keys, v->keys + v->n_keys);
 	c->pos_off.assign(v->pos_off, v->pos_off + v->n_keys + 1);
@@ -265,6 +266,7 @@ static wm_gpu_ctx_s *index_build(const char *who, const char *ref_fn, const char
 		if (group.size() >= ((size_t)1 << 30)) flush();
 	}
 	flush();
+	set_name_order(&H);
 	ws.release(); d_ascii.release(); d_pk.release(); d_nm.release(); cudaFree(d_table);
 	// one array in position order, then sort + CSR on the device
 	wm128_dev *d_all = wm_dev_alloc<wm128_dev>(n_mz_total + 1);
@@ -337,6 +339,7 @@ extern "C" int wm_gpu_map_batch(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, int n_s
 	#pragma omp parallel for schedule(dynamic, 16) num_threads(n_threads > 0 ? n_threads : 1)
 	for (int i = 0; i < n_seq; ++i) {
 		store[i].name = names && names[i] ? names[i] : "";
+		store[i].has_name = names && names[i];
 		store[i].seq.assign(seqs[i], lens[i]);
 		reads[i] = &store[i];
 	}
@@ -365,8 +368,7 @@ extern "C" wm_reg1_t *wm_map(wm_gpu_ctx_s *c, int l_seq, const char *seq, int *n
 {
 	int32_t n_reg = 0, rl = 0, fg = 0, len = l_seq;
 	wm_reg1_t *reg = 0;
-	const char *nm = name ? name : "";
-	wm_gpu_map_batch(c, opt, 1, &nm, &seq, &len, &n_reg, &reg, &rl, &fg, 1);
+	wm_gpu_map_batch(c, opt, 1, &name, &seq, &len, &n_reg, &reg, &rl, &fg, 1); // name == NULL: qname == 0
 	if (b) b->rep_len = rl, b->frag_gap = fg;
 	*n_regs = n_reg;
 	return reg;

@@ -20,6 +20,9 @@ void wm_ksw_ll_launch(const wm_ll_job *d_jobs, int n, const uint8_t *d_seq, cons
 
 using namespace wmh;
 
+static_assert(WM_SKIP_NO_DIAG == SKIP_NO_DIAG && WM_SKIP_NO_DUAL == SKIP_NO_DUAL && WM_SKIP_FOR_ONLY == SKIP_FOR_ONLY &&
+              WM_SKIP_REV_ONLY == SKIP_REV_ONLY && WM_SKIP_NAME_EQ == SKIP_NAME_EQ, "seed filter bits");
+
 // ---- small data-movement kernels ----
 // Masked copy of a window (src/map.c:795-801: covered bases become ambiguous) as a packed sequence of its own: one thread
 // per 32 bases takes the unaligned source windows and sets the flags of the covered bases.
@@ -94,7 +97,7 @@ struct GpuBackendImpl {
 	char *h_stage = 0; size_t h_stage_cap = 0; // pinned staging buffer of begin_batch
 	// workspaces
 	wm_sketch_ws sk; wm_seed_ws sd, sd2; wm_chain_ws ch; wm_extd2_ws dpws;
-	wm_dbuf masked_pk, masked_nm, mask_tasks, mask_toff, mask_pool, qlen_buf, pre_buf, cat_tasks, cat_toff, cat_a, set_id, off_buf, nb_off, nu_off, b_out, u_out;
+	wm_dbuf masked_pk, masked_nm, mask_tasks, mask_toff, mask_pool, qlen_buf, skip_buf, pre_buf, cat_tasks, cat_toff, cat_a, set_id, off_buf, nb_off, nu_off, b_out, u_out;
 	wm_dbuf nc_buf, scan_tmp, coop_ids, g_jobs, g_joff, seq_pool, dp_jobs, bt, ez, cig, cig_off, cig_out, ll_jobs, ll_scr, ll_out, mat;
 	// host result pools
 	std::vector<uint32_t> h_mzpos; std::vector<int64_t> h_mz_off; std::vector<int32_t> h_rep;
@@ -118,8 +121,11 @@ public:
 		if (g.owns_index) {
 			cudaFree((void*)g.ix.keys); cudaFree((void*)g.ix.pos_off); cudaFree((void*)g.ix.pos); cudaFree((void*)g.ix.S);
 			cudaFree((void*)g.ix.ht_key); cudaFree((void*)g.ix.ht_val); cudaFree((void*)g.bf.table);
+			cudaFree((void*)g.ix.seq_len); cudaFree((void*)g.ix.name_rank);
 		}
 		if (g.st) cudaStreamDestroy(g.st);
+		// this thread's workspace allocations must not go on to the stream just destroyed (wm_dbuf_use_stream)
+		if (wm_dbuf_stream == g.st) wm_dbuf_stream = 0, wm_dbuf_async = false;
 	}
 	void begin_batch(const std::vector<const wm_read*> &reads) override;
 	void set_resident_pool(const char *device_ascii) override { g.resident_pool = device_ascii; }
@@ -252,8 +258,16 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 		for (int i = 0; i < ns; ++i) qlen[i] = skt[i].len;
 		int32_t *d_qlen = (int32_t*)g.qlen_buf.need(sizeof(int32_t) * ns);
 		WM_CUDA_CHECK(wm_memcpy_async(d_qlen, qlen.data(), sizeof(int32_t) * ns, cudaMemcpyHostToDevice, st));
+		std::vector<uint2> skip(ns); // the seed filter of the pass' tasks; none when no task has a bit set
+		bool any_skip = false;
+		for (int i = 0; i < ns; ++i) { skip[i] = make_uint2(tasks[ids[i]].skip, tasks[ids[i]].name_lt); any_skip |= skip[i].x != 0; }
+		uint2 *d_skip = 0;
+		if (any_skip) {
+			d_skip = (uint2*)g.skip_buf.need(sizeof(uint2) * ns);
+			WM_CUDA_CHECK(wm_memcpy_async(d_skip, skip.data(), sizeof(uint2) * ns, cudaMemcpyHostToDevice, st));
+		}
 		std::vector<int64_t> a_off(ns + 1);
-		wm_seed_run(sdp[pass], g.ix, (const wm128_dev*)g.sk.mz.p, (const int64_t*)g.sk.mz_off.p, n_mz, ns, d_qlen, max_occ, a_off.data(), st);
+		wm_seed_run(sdp[pass], g.ix, (const wm128_dev*)g.sk.mz.p, (const int64_t*)g.sk.mz_off.p, n_mz, ns, d_qlen, max_occ, a_off.data(), st, d_skip);
 		d_seed_a[pass] = (wm128_dev*)sdp[pass]->a.p;
 		// small per-task results
 		std::vector<int32_t> rep(ns);
@@ -650,7 +664,18 @@ Backend *gpu_backend_create_dev(const wm_host_idx *hidx, uint64_t *d_keys, int64
 	uint8_t *d_bt = wm_dev_alloc<uint8_t>(bloom_bits / 8 + 16);
 	WM_CUDA_CHECK(cudaMemcpy(d_S, hidx->S.data(), sizeof(uint32_t) * hidx->S.size(), cudaMemcpyHostToDevice));
 	WM_CUDA_CHECK(cudaMemcpy(d_bt, bloom_table, bloom_bits / 8, cudaMemcpyHostToDevice));
+	// lengths and name ranks of the sequences for the seed filter of -D / --dual=no (the ranks of hidx, or worked out here
+	// from its names when a caller did not set its name order)
+	const size_t n_seq = hidx->len.size();
+	uint32_t *d_len = wm_dev_alloc<uint32_t>(n_seq + 1), *d_rank = wm_dev_alloc<uint32_t>(n_seq + 1);
+	std::vector<uint32_t> rank = hidx->name_rank;
+	if (rank.size() != n_seq) { wm_host_idx t; t.name = hidx->name; set_name_order(&t); rank.swap(t.name_rank); }
+	if (n_seq) {
+		WM_CUDA_CHECK(cudaMemcpy(d_len, hidx->len.data(), sizeof(uint32_t) * n_seq, cudaMemcpyHostToDevice));
+		WM_CUDA_CHECK(cudaMemcpy(d_rank, rank.data(), sizeof(uint32_t) * n_seq, cudaMemcpyHostToDevice));
+	}
 	memset(&g.ix, 0, sizeof(g.ix));
+	g.ix.seq_len = d_len, g.ix.name_rank = d_rank;
 	g.ix.k = hidx->k, g.ix.w = hidx->w, g.ix.n_seq = (uint32_t)hidx->len.size();
 	g.ix.n_keys = n_keys, g.ix.keys = d_keys, g.ix.pos_off = d_poff, g.ix.pos = d_pos, g.ix.S = d_S;
 	wm_idx_dev_build_ht(&g.ix, g.st);

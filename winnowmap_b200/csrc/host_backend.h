@@ -16,13 +16,27 @@ struct MapWin { int32_t read, wb, wl; }; // a query window: bases [wb, wb+wl) of
 
 enum { SEED_MASKED = 1, SEED_NO_SKETCH = 2 };
 
+// The per-occurrence filter of skip_seed (src/map.c:132-154) as integer tests.  SKIP_NO_DIAG / SKIP_NO_DUAL are set only
+// when the read has a name; with the index names in strcmp order (wm_host_idx::name_rank), for the occurrence's rid:
+//   strcmp(qname, name[rid]) > 0   <=>  name_rank[rid] < name_lt
+//   strcmp(qname, name[rid]) == 0  <=>  SKIP_NAME_EQ && name_rank[rid] == name_lt
+enum { SKIP_NO_DIAG = 1, SKIP_NO_DUAL = 2, SKIP_FOR_ONLY = 4, SKIP_REV_ONLY = 8, SKIP_NAME_EQ = 16 };
+
 struct SeedTask {
 	MapWin win;
 	int32_t flags;      // SEED_MASKED: sketch a copy whose covered bases are 'N' (src/map.c:793-803); SEED_NO_SKETCH: chain `pre` only
 	int32_t chain_set;  // which of the two chaining parameter sets applies (stage-1/fallback vs stage-2)
 	int32_t n_mask; int64_t mask_off; // covered intervals [s,e) as int32 pairs in the mask pool
 	int32_t n_pre; int64_t pre_off;   // anchors from stage 1 (sorted) in the pre pool (src/map.c:742-774)
+	// the filter of the fresh look-ups (the `pre` anchors went through it in stage 1): SKIP_* bits (0: every occurrence is
+	// kept, no filter runs) and the number of index names strictly less than the read's name
+	uint32_t skip = 0, name_lt = 0;
 };
+
+// name_rank / name_sorted of the index (one sort of the names per index)
+void set_name_order(wm_host_idx *mi);
+// SKIP_* bits and name_lt of one read under the mapping flags `flag` (mi's name order must be set when -D / --dual=no is on)
+uint32_t skip_bits(const wm_host_idx *mi, int64_t flag, const wm_read *rd, uint32_t *name_lt);
 
 struct ChainParams { // arguments of mm_chain_dp (src/chain.c:22)
 	int32_t max_dist_x, min_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc;

@@ -94,6 +94,38 @@ ChainParams chain_params(const wm_mapopt_t *o, const wm_mapopt_t *base, int qlen
 
 } // namespace
 
+void set_name_order(wm_host_idx *mi)
+{ // strcmp compares bytes as unsigned char, as std::string::compare does: equal names get equal ranks
+	const uint32_t n = (uint32_t)mi->name.size();
+	std::vector<uint32_t> &s = mi->name_sorted, &rank = mi->name_rank;
+	s.resize(n), rank.resize(n);
+	for (uint32_t i = 0; i < n; ++i) s[i] = i;
+	std::stable_sort(s.begin(), s.end(), [&](uint32_t a, uint32_t b) { return strcmp(mi->name[a].c_str(), mi->name[b].c_str()) < 0; });
+	for (uint32_t i = 0; i < n; ++i)
+		rank[s[i]] = i > 0 && mi->name[s[i]] == mi->name[s[i - 1]] ? rank[s[i - 1]] : i;
+}
+
+uint32_t skip_bits(const wm_host_idx *mi, int64_t flag, const wm_read *rd, uint32_t *name_lt)
+{ // skip_seed (src/map.c:132-154), the parts that depend on the read only
+	uint32_t b = 0;
+	*name_lt = 0;
+	if (flag & WM_F_FOR_ONLY) b |= SKIP_FOR_ONLY;
+	if (flag & WM_F_REV_ONLY) b |= SKIP_REV_ONLY;
+	if (!rd->has_name || !(flag & (WM_F_NO_DIAG | WM_F_NO_DUAL))) return b;
+	if (mi->name_sorted.size() != mi->name.size()) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: the index's name order is not set (set_name_order)\n");
+		exit(1);
+	}
+	if (flag & WM_F_NO_DIAG) b |= SKIP_NO_DIAG;
+	if (flag & WM_F_NO_DUAL) b |= SKIP_NO_DUAL;
+	const char *q = rd->name.c_str();
+	const std::vector<uint32_t> &s = mi->name_sorted;
+	const size_t lt = std::partition_point(s.begin(), s.end(), [&](uint32_t r) { return strcmp(mi->name[r].c_str(), q) < 0; }) - s.begin();
+	if (lt < s.size() && mi->name[s[lt]] == rd->name) b |= SKIP_NAME_EQ;
+	*name_lt = (uint32_t)lt;
+	return b;
+}
+
 void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads,
                std::vector<std::vector<wm_reg1_t>> &regs_out, std::vector<int> &rep_len_out, std::vector<int> &frag_gap_out, int n_threads, MapStats *st)
 {
@@ -103,8 +135,8 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	frag_gap_out.assign(n_reads, 0);
 	if (n_reads == 0) return;
 	if (n_threads < 1) n_threads = 1;
-	if (opt->flag & (WM_F_SPLICE | WM_F_SR | WM_F_HEAP_SORT | WM_F_NO_DIAG | WM_F_NO_DUAL | WM_F_FOR_ONLY | WM_F_REV_ONLY)) {
-		fprintf(stderr, "[ERROR] winnowmap-b200: splice/sr/heap-sort/-X/--for-only/--rev-only modes are outside the accelerated path\n");
+	if (opt->flag & (WM_F_SPLICE | WM_F_SR | WM_F_HEAP_SORT)) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: splice/sr/heap-sort modes are outside the accelerated path\n");
 		exit(1);
 	}
 	// options the reference honours on this path that are not implemented here are refused, not silently ignored
@@ -144,6 +176,11 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	sc.q = opt->q, sc.e = opt->e, sc.q2 = opt->q2, sc.e2 = opt->e2;
 
 	std::vector<ReadState> rs(n_reads);
+	std::vector<uint32_t> skip(n_reads, 0), name_lt(n_reads, 0); // the seed filter of every read (-D, --dual=no, --for-only, --rev-only)
+	if (opt->flag & (WM_F_NO_DIAG | WM_F_NO_DUAL | WM_F_FOR_ONLY | WM_F_REV_ONLY)) {
+		#pragma omp parallel for schedule(static) num_threads(n_threads)
+		for (int i = 0; i < n_reads; ++i) skip[i] = skip_bits(mi, opt->flag, reads[i], &name_lt[i]);
+	}
 	std::vector<Cursor> cursors;
 	std::vector<int> levels;
 	for (int sub_len = opt2.minPrefixLength; sub_len <= opt2.maxPrefixLength; sub_len = (int)((float)sub_len * opt2.prefixIncrementFactor)) {
@@ -312,6 +349,7 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 				M.opt = &opt2, M.chain_set = 0, M.est_err = true;
 				SeedTask t;
 				t.win = M.win, t.flags = 0, t.chain_set = 0, t.n_mask = 0, t.mask_off = 0, t.n_pre = 0, t.pre_off = 0;
+				t.skip = skip[C.read], t.name_lt = name_lt[C.read];
 				tasks[k] = t;
 			}
 		}
@@ -384,6 +422,7 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		M.est_err = false;
 		SeedTask t;
 		t.win = M.win, t.n_mask = 0, t.mask_off = 0, t.n_pre = 0, t.pre_off = 0;
+		t.skip = skip[i], t.name_lt = name_lt[i];
 		if (!a.empty()) {
 			int unmapped = 0;
 			for (int k = 0; k < R.qlen; ++k) unmapped += R.mapped[k] == 0;

@@ -64,6 +64,9 @@ struct wm_host_idx {
 	std::vector<uint32_t> len;
 	std::vector<uint64_t> offset;
 	std::vector<uint32_t> S; // 4-bit packed, mm_seq4_set layout (src/mmpriv.h:29-30)
+	// strcmp order of the names (set_name_order): the name tests of -D / --dual=no become integer comparisons.
+	// name_rank[rid] = number of names strictly less than name[rid]; name_sorted: the rids in that order
+	std::vector<uint32_t> name_rank, name_sorted;
 	inline int base(uint64_t i) const { return S[i >> 3] >> ((i & 7) << 2) & 0xf; }
 	// mm_idx_getseq (src/index.c:161-171)
 	int getseq(uint32_t rid, uint32_t st, uint32_t en, uint8_t *seq) const {
@@ -88,4 +91,5 @@ struct wm_read {
 	std::string seq;   // ASCII
 	std::string qual;
 	int64_t dev_off = -1; // >= 0: the bases are also resident in the device pool given to Backend::set_resident_pool, at this offset
+	bool has_name = true; // false: mm_map with qname == 0 (the name tests of -D / --dual=no are off; `name` is "")
 };

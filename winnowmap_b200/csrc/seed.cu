@@ -74,10 +74,14 @@ __global__ void wm_seed_lookup_kernel(wm_idx_dev ix, const wm128_dev *__restrict
 	mz_task[m] = lo;
 }
 
-// pass 2: one thread per anchor (src/map.c:233-249; skip_seed() is a no-op without -D/-X/--for-only/--rev-only)
+// pass 2: one thread per anchor (src/map.c:233-249).  FILTER: skip_seed (src/map.c:132-154) with the per-task bits of the
+// seed filter (skip[t].x: WM_SKIP_* bits, .y: index names less than the read's name); keep[j] = 0 drops the occurrence.  Without
+// -D / --dual=no / --for-only / --rev-only skip_seed() never skips: the FILTER = false instance runs and nothing is compacted.
+template <bool FILTER>
 __global__ void wm_seed_expand_kernel(wm_idx_dev ix, const wm128_dev *__restrict__ mz, int64_t n_mz, const int64_t *__restrict__ a_off,
                                       const uint64_t *__restrict__ list_off, const uint8_t *__restrict__ tandem, const int32_t *__restrict__ mz_task,
-                                      const int32_t *__restrict__ qlen, int64_t n_a, wm128_dev *__restrict__ a)
+                                      const int32_t *__restrict__ qlen, int64_t n_a, wm128_dev *__restrict__ a,
+                                      const uint2 *__restrict__ skip, int32_t *__restrict__ keep)
 {
 	const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if (j >= n_a) return;
@@ -97,7 +101,39 @@ __global__ void wm_seed_expand_kernel(wm_idx_dev ix, const wm128_dev *__restrict
 	}
 	o.y |= (uint64_t)(p.y >> 32) << 48; // MM_SEED_SEG_SHIFT
 	if (tandem[lo]) o.y |= 1ULL << 42;   // MM_SEED_TANDEM
+	if (FILTER) {
+		const int t = mz_task[lo];
+		const uint2 sk = skip[t];
+		const bool fwd = (r & 1) == (q_pos & 1);
+		bool drop = false;
+		if (sk.x & (WM_SKIP_NO_DIAG | WM_SKIP_NO_DUAL)) {
+			const uint32_t rid = (uint32_t)(r >> 32), rank = ix.name_rank[rid];
+			// strcmp(qname, name) == 0 and the sequence is as long as the window (not the read: src/map.c:364, :813)
+			if ((sk.x & WM_SKIP_NO_DIAG) && (sk.x & WM_SKIP_NAME_EQ) && rank == sk.y && (int)ix.seq_len[rid] == qlen[t]) {
+				if ((uint32_t)rpos == q_pos >> 1) drop = true; // the diagonal
+				else if (fwd) o.y |= 1ULL << 43;              // MM_SEED_SELF
+			}
+			if ((sk.x & WM_SKIP_NO_DUAL) && rank < sk.y) drop = true; // strcmp(qname, name) > 0
+		}
+		if ((sk.x & WM_SKIP_FOR_ONLY) && !fwd) drop = true;
+		if ((sk.x & WM_SKIP_REV_ONLY) && fwd) drop = true;
+		keep[j] = drop ? 0 : 1;
+	}
 	a[j] = o;
+}
+
+// the seed filter's compaction, stable (the kept anchors keep their order, as collect_seed_hits writes them, so the tie-exact
+// sort sees what radix_sort_128x sees): one thread per anchor, then one per task offset, which moves to its rank among the kept
+__global__ void wm_seed_compact_kernel(const wm128_dev *__restrict__ a_raw, const int32_t *__restrict__ keep, const int64_t *__restrict__ keep_off,
+                                       int64_t n_a, int64_t *__restrict__ task_a_off, int n_tasks, wm128_dev *__restrict__ a)
+{
+	const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (j < n_a) {
+		if (keep[j]) a[keep_off[j]] = a_raw[j];
+	} else if (j - n_a <= n_tasks) {
+		const int t = (int)(j - n_a);
+		task_a_off[t] = keep_off[task_a_off[t]];
+	}
 }
 
 // pass 3: one thread per task: rep_len (src/map.c:106-127), kept-minimizer count, anchor offsets
@@ -708,8 +744,8 @@ void wm_anchor_sort_run(wm_seed_ws *ws, wm128_dev *d_a, const int64_t *d_off, co
 // On return: ws->a (anchors), ws->task_a_off (device, n_tasks+1), ws->rep_len, ws->n_mini_pos, ws->mini_pos;
 // h_task_a_off (host, n_tasks+1) receives the anchor offsets.
 void wm_seed_run(wm_seed_ws *ws, const wm_idx_dev &ix, const wm128_dev *d_mz, const int64_t *d_mz_off, int64_t n_mz, int n_tasks,
-                 const int32_t *d_qlen, int max_occ, int64_t *h_task_a_off, cudaStream_t st)
-{
+                 const int32_t *d_qlen, int max_occ, int64_t *h_task_a_off, cudaStream_t st, const uint2 *d_skip)
+{ // d_skip: the seed filter's bits per task, or null when no task filters (then no filter kernel runs)
 	for (int i = 0; i <= n_tasks; ++i) h_task_a_off[i] = 0;
 	int64_t *d_task_a_off = (int64_t*)ws->task_a_off.need(sizeof(int64_t) * (n_tasks + 1));
 	int32_t *d_rep = (int32_t*)ws->rep_len.need(sizeof(int32_t) * (n_tasks + 1));
@@ -736,15 +772,33 @@ void wm_seed_run(wm_seed_ws *ws, const wm_idx_dev &ix, const wm128_dev *d_mz, co
 	WM_CUDA_CHECK(wm_memcpy_async(&n_a, d_aoff + n_mz, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
 	wm_stream_sync(st);
 	ws->n_a = n_a;
-	wm128_dev *d_a = (wm128_dev*)ws->a.need(sizeof(wm128_dev) * (n_a + 1));
-	if (n_a > 0) {
-		wm_count_launch(); wm_seed_expand_kernel<<<(unsigned)((n_a + 127) / 128), 128, 0, st>>>(ix, d_mz, n_mz, d_aoff, d_loff, d_td, d_mtask, d_qlen, n_a, d_a);
+	wm128_dev *d_a = (wm128_dev*)ws->a.need(sizeof(wm128_dev) * (n_a + 1)); // (with the filter: the bound before it)
+	const bool filter = d_skip && n_a > 0;
+	if (filter) {
+		// the anchors before compaction and their keep flags go to the sort's per-anchor scratch (sort_tmp, sort_idx: dead until the
+		// sort below, and sized for at least these n_a anchors there); only the scan of the flags takes a buffer of its own
+		wm128_dev *d_raw = (wm128_dev*)ws->sort_tmp.need(sizeof(wm128_dev) * (n_a + 1));
+		int32_t *d_keep = (int32_t*)ws->sort_idx.need(sizeof(int32_t) * (n_a + 1));
+		int64_t *d_koff = (int64_t*)ws->keep_off.need(sizeof(int64_t) * (n_a + 1));
+		wm_count_launch(); wm_seed_expand_kernel<true><<<(unsigned)((n_a + 127) / 128), 128, 0, st>>>(ix, d_mz, n_mz, d_aoff, d_loff, d_td, d_mtask, d_qlen, n_a, d_raw, d_skip, d_keep);
+		WM_CUDA_CHECK(cudaGetLastError());
+		wm_count_launch(); wm_seed_task_kernel<<<(n_tasks + 1 + 127) / 128, 128, 0, st>>>(d_mz, d_mz_off, d_aoff, d_nocc, max_occ, n_tasks, d_rep, d_nmp, d_task_a_off, d_mpos);
+		WM_CUDA_CHECK(cudaGetLastError());
+		int64_t *d_tmp2 = (int64_t*)ws->scan_tmp.need(sizeof(int64_t) * wm_scan_tmp_elems(std::max(n_mz, n_a)));
+		wm_exclusive_scan(d_keep, n_a, d_koff, d_tmp2, st);
+		wm_count_launch(); wm_seed_compact_kernel<<<(unsigned)((n_a + n_tasks + 1 + 127) / 128), 128, 0, st>>>(d_raw, d_keep, d_koff, n_a, d_task_a_off, n_tasks, d_a);
+		WM_CUDA_CHECK(cudaGetLastError());
+	} else {
+		if (n_a > 0) {
+			wm_count_launch(); wm_seed_expand_kernel<false><<<(unsigned)((n_a + 127) / 128), 128, 0, st>>>(ix, d_mz, n_mz, d_aoff, d_loff, d_td, d_mtask, d_qlen, n_a, d_a, 0, 0);
+			WM_CUDA_CHECK(cudaGetLastError());
+		}
+		wm_count_launch(); wm_seed_task_kernel<<<(n_tasks + 1 + 127) / 128, 128, 0, st>>>(d_mz, d_mz_off, d_aoff, d_nocc, max_occ, n_tasks, d_rep, d_nmp, d_task_a_off, d_mpos);
 		WM_CUDA_CHECK(cudaGetLastError());
 	}
-	wm_count_launch(); wm_seed_task_kernel<<<(n_tasks + 1 + 127) / 128, 128, 0, st>>>(d_mz, d_mz_off, d_aoff, d_nocc, max_occ, n_tasks, d_rep, d_nmp, d_task_a_off, d_mpos);
-	WM_CUDA_CHECK(cudaGetLastError());
 	WM_CUDA_CHECK(wm_memcpy_async(h_task_a_off, d_task_a_off, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyDeviceToHost, st));
 	wm_stream_sync(st);
+	ws->n_a = h_task_a_off[n_tasks];
 	wm_anchor_sort_run(ws, d_a, d_task_a_off, h_task_a_off, n_tasks, st);
 }
 

@@ -29,6 +29,7 @@ class MapOpt(C.Structure):  # wm_mapopt_t == mm_mapopt_t (reference src/minimap.
 
 
 F_CIGAR, F_OUT_SAM, F_OUT_CG, F_NO_PRINT_2ND, F_PAF_NO_HIT = 0x004, 0x008, 0x020, 0x4000, 0x8000000
+F_NO_DIAG, F_NO_DUAL, F_NO_LJOIN, F_FOR_ONLY, F_REV_ONLY, F_ALL_CHAINS = 0x001, 0x002, 0x400, 0x100000, 0x200000, 0x800000
 I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
 
 STAT_NAMES = ("n_reads", "n_bases", "n_minimaps", "n_chained", "n_dp_jobs", "n_ll_jobs", "n_rounds", "t_seed", "t_dp", "t_host",
@@ -62,9 +63,10 @@ def _setup(L):
 F_OUT_SAM = 0x008
 
 
-def make_options(preset=None, cigar=True, sam=False):
+def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, all_vs_all=False, strand=None):
     """mm_set_opt(0) then mm_set_opt(preset) (reference main.c:144-159); -c sets MM_F_OUT_CG|MM_F_CIGAR, -a sets
-    MM_F_OUT_SAM|MM_F_CIGAR (main.c)."""
+    MM_F_OUT_SAM|MM_F_CIGAR (main.c).  Self and all-vs-all mapping: no_diag is -D, dual=False is --dual=no, all_vs_all
+    is -X (-D -P --no-long-join --dual=no); strand="for" / "rev" is --for-only / --rev-only."""
     L = _setup(lib())
     io, mo = IdxOpt(), MapOpt()
     L.wm_set_opt(None, C.byref(io), C.byref(mo))
@@ -74,6 +76,16 @@ def make_options(preset=None, cigar=True, sam=False):
         mo.flag |= F_OUT_SAM | F_CIGAR
     elif cigar:
         mo.flag |= F_OUT_CG | F_CIGAR
+    if no_diag:
+        mo.flag |= F_NO_DIAG
+    if not dual:
+        mo.flag |= F_NO_DUAL
+    if all_vs_all:
+        mo.flag |= F_ALL_CHAINS | F_NO_DIAG | F_NO_DUAL | F_NO_LJOIN
+    if strand is not None:
+        if strand not in ("for", "rev", "both"):
+            raise ValueError(f"strand must be 'for', 'rev' or 'both', not {strand!r}")
+        mo.flag |= {"for": F_FOR_ONLY, "rev": F_REV_ONLY, "both": 0}[strand]
     rc = L.wm_check_opt(C.byref(io), C.byref(mo))
     if rc < 0:
         raise ValueError(f"mm_check_opt-style validation failed: {rc}")
@@ -82,11 +94,14 @@ def make_options(preset=None, cigar=True, sam=False):
 
 class Mapper:
     """winnowmap [-W rep.txt] -x preset [-H] -c ref.fa reads.fa  on one GPU.  hpc=True is -H: the index and the reads are
-    sketched with homopolymer-compressed k-mers (reference src/main.c:166).  A blob carries its own flag."""
+    sketched with homopolymer-compressed k-mers (reference src/main.c:166).  A blob carries its own flag.  no_diag, dual,
+    all_vs_all and strand are the self / all-vs-all and single-strand options of make_options (-D, --dual, -X,
+    --for-only / --rev-only): Mapper(reads, preset="map-ont", all_vs_all=True).map_file(reads, out) computes overlaps."""
 
-    def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False):
+    def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
+                 no_diag=False, dual=True, all_vs_all=False, strand=None):
         self.L = _setup(lib())
-        self.io, self.mo = make_options(preset, cigar, sam)
+        self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand)
         if hpc:
             self.io.flag |= I_HPC
         self.n_threads = n_threads or max(1, min(64, (os.cpu_count() or 2) // 2))
