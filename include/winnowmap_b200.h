@@ -219,7 +219,8 @@ typedef struct { /* mm_mapopt_t, src/minimap.h:112-176 */
 } wm_mapopt_t;
 
 
-/* mm_set_opt / mm_check_opt (src/options.c:89,133): same presets, same return codes */
+/* mm_set_opt / mm_check_opt (src/options.c:89,133): same presets, same return codes, plus -7 for two gap pairs whose
+   int8 lanes in the reference's ksw_extd2_sse can wrap (-A + q + 2e > 128), which the device fill does not reproduce */
 int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo);
 int wm_check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo);
 int wm_sizeof_mapopt(void);

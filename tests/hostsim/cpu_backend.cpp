@@ -156,10 +156,16 @@ public:
 	}
 };
 
-static int g_gap_override[4] = {0, 0, 0, 0}; // -O / -E of the next run (0 = keep the preset's)
-extern "C" void wmt_set_gap(int q, int e, int q2, int e2) { g_gap_override[0] = q, g_gap_override[1] = e, g_gap_override[2] = q2, g_gap_override[3] = e2; }
+// -A / -B / --score-N / -O / -E of the next run; a negative entry keeps the preset's value
+static int g_scoring_override[7] = {-1, -1, -1, -1, -1, -1, -1};
+extern "C" void wmt_set_scoring(int a, int b, int sc_ambi, int q, int e, int q2, int e2)
+{
+	const int v[7] = {a, b, sc_ambi, q, e, q2, e2};
+	memcpy(g_scoring_override, v, sizeof(v));
+}
+extern "C" void wmt_set_gap(int q, int e, int q2, int e2) { wmt_set_scoring(-1, -1, -1, q > 0 ? q : -1, e > 0 ? e : -1, q2 > 0 ? q2 : -1, e2 > 0 ? e2 : -1); }
 
-// the options of one run: preset, -c or -a, extra output flags and the one-shot -O / -E override
+// the options of one run: preset, -c or -a, extra output flags and the one-shot scoring override
 static int run_opts(const char *preset, int sam, int64_t extra_flags, wm_idxopt_t &io, wm_mapopt_t &mo)
 {
 	set_opt(0, &io, &mo);
@@ -167,8 +173,9 @@ static int run_opts(const char *preset, int sam, int64_t extra_flags, wm_idxopt_
 	if (sam) mo.flag |= WM_F_OUT_SAM | WM_F_CIGAR; // -a (src/main.c)
 	else mo.flag |= WM_F_OUT_CG | WM_F_CIGAR;      // -c
 	mo.flag |= extra_flags;                        // --cs / --cs=long / --MD (src/main.c:227,249-266)
-	if (g_gap_override[0] > 0) mo.q = g_gap_override[0], mo.e = g_gap_override[1], mo.q2 = g_gap_override[2], mo.e2 = g_gap_override[3]; // -O / -E (src/main.c)
-	g_gap_override[0] = 0; // one shot
+	int *const field[7] = {&mo.a, &mo.b, &mo.sc_ambi, &mo.q, &mo.e, &mo.q2, &mo.e2}; // src/main.c: -A, -B, --score-N, -O, -E
+	for (int i = 0; i < 7; ++i) if (g_scoring_override[i] >= 0) *field[i] = g_scoring_override[i];
+	for (int i = 0; i < 7; ++i) g_scoring_override[i] = -1; // one shot
 	return check_opt(&io, &mo) < 0 ? -2 : 0;
 }
 

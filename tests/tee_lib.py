@@ -33,6 +33,7 @@ def load(so):
     L = C.CDLL(so)
     s, i, i64, p = C.c_char_p, C.c_int, C.c_int64, C.c_void_p
     L.wmt_set_gap.argtypes = [i, i, i, i]
+    L.wmt_set_scoring.argtypes = [i] * 7
     L.wmt_tee_map_file.argtypes = [s, s, s, s, s, i, i, i64, i, i, s]
     L.wmt_tee_seed_chain.argtypes = [s, s, i, i, i, i, i, i, p, p, i, p, i, p, p, p, i, s]
     L.wmt_tee_align.argtypes = [s, i, i, i, i, i64, i, p, p, i, p, i, p, i, p, p, p, s]
@@ -353,13 +354,27 @@ def crafted_ll_jobs(wins, contigs, rng, n=60):
     return rows
 
 
-SCORINGS = {  # (match, mismatch, q, e, q2, e2): map-ont, asm20-like, one gap pair (ksw_extz2), and a mismatch above 2(q + e),
-    # for which ksw_extd2_sse returns before the sweep (src/ksw2_extd2_sse.c:92; -B13 with map-ont's gaps)
-    "map-ont": (2, 4, 4, 2, 24, 1),
-    "asm20": (1, 4, 6, 2, 26, 1),
-    "single": (2, 4, 4, 2, 4, 2),
-    "early-out": (1, 13, 4, 2, 24, 1),
+SCORINGS = {  # (-A, -B, -O q, -E e, -O q2, -E e2, --score-N): every scoring class the mapper accepts, each pinned at every layer
+    "map-ont": (2, 4, 4, 2, 24, 1, 1),
+    "asm20": (1, 4, 6, 2, 26, 1, 1),
+    "single": (2, 4, 4, 2, 4, 2, 1),          # one gap pair: ksw_extz2 (src/align.c:328-331)
+    # a mismatch above 2(q + e): ksw_extd2_sse returns before the sweep (src/ksw2_extd2_sse.c:92)
+    "early-out": (1, 13, 4, 2, 24, 1, 1),
+    "asm10": (1, 9, 16, 2, 41, 1, 1),
+    # gap sum 124; e - e2 = 2: long_thres 20, long_diff -3 (every scoring above has e - e2 = 1 and long_diff -2)
+    "asm5": (1, 19, 39, 3, 81, 1, 1),
+    "long_inc": (2, 5, 4, 3, 25, 1, 1),       # the ++long_thres branch (src/ksw2_extd2_sse.c:95-96): 9 -> 10
+    # gap sum exactly 127 (the option check's limit) and a mismatch of exactly 2(q + e): the last scoring that still sweeps
+    "limit": (1, 86, 40, 3, 83, 1, 1),
+    "single_asm5": (1, 19, 39, 3, 39, 3, 1),  # ksw_extz2 with a large mismatch
+    "N0": (2, 4, 4, 2, 24, 1, 0),             # N cells score -e2 in extd2, -e in extz2 (src/ksw2_extd2_sse.c:79)
+    "N3": (2, 4, 4, 2, 24, 1, 3),
+    "N13": (2, 4, 4, 2, 24, 1, 13),           # the N entries of the matrix, not the mismatch, make the early return
+    "match_hi": (20, 4, 4, 2, 24, 1, 1),
 }
+# -A + q + 2e > 128: the reference's int8 lanes wrap (src/ksw2_extd2_sse.c:52-58), the device fill does not.  The oracle
+# follows the reference here; the mapper refuses the scoring (check_opt returns -7).
+REFUSED_SCORINGS = {"wrap_probe": (100, 4, 40, 3, 83, 1, 1)}
 
 
 def write_fasta(path, seqs):

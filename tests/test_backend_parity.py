@@ -36,6 +36,9 @@ SHAPES = {
     "hifi_small": ["seed.pre", "seed.mixed_set_calls"],  # no masked task, no sort #3, no ll, no coop job
     "ont_tandem": ["seed.pre", "seed.mixed_set_calls"],  # no masked task, no sort #3, no ll, no coop job
     "asm20_small": ["seed.pre"],                         # every read has stage-1 anchors: one chain set; no mask, sort #3, ll, coop
+    "asm5_small": ["seed.pre", "ll.jobs"],               # one chain set; no mask, sort #3, coop
+    "asm10_small": ["seed.pre", "ll.jobs"],              # one chain set; no mask, sort #3, coop
+    "ont_sv_long_inc": ["seed.pre", "seed.masked", "sort3.le2048", "seed.mixed_set_calls", "ll.jobs", "dp.coop_jobs"],  # as ont_sv
     "hpc_clr": ["dp.coop_jobs"],                         # one pass: no stage-1 anchors, so no mask, sort #3 or second set; no ll
     "hpc_ont_small": ["seed.pre", "seed.mixed_set_calls", "dp.coop_jobs"],  # no masked task, no sort #3, no ll
 }
@@ -50,7 +53,7 @@ so, case, rep = sys.argv[1], json.loads(sys.argv[2]), sys.argv[3]
 L = T.load(so)
 kind = case.pop("kind")
 if kind == "map":
-    L.wmt_set_gap(*case["gap"])
+    L.wmt_set_scoring(*case["scoring"])
     rc = L.wmt_tee_map_file(case["ref"].encode(), case["w"].encode() if case["w"] else None, case["preset"].encode(), case["reads"].encode(),
                             case["out"].encode(), 8, case["hpc"], case["budget"], T.DEV_GPU, 0, rep.encode())
     sys.exit(0 if rc == 0 else 3)
@@ -64,9 +67,9 @@ if kind == "seed":
 else:
     rng = np.random.default_rng(11)
     wins = T.crafted_dp_windows(reads)
-    a, b, q, e, q2, e2 = T.SCORINGS[case["scoring"]]
+    a, b, q, e, q2, e2, sc_ambi = T.SCORINGS[case["scoring"]]
     T.align(L, rep, ref, 15, 10, reads, wins, T.crafted_dp_jobs(origin, wins, rng), T.crafted_ll_jobs(wins, contigs, rng),
-            ol.simple_mat(a, b, 1), (q, e, q2, e2), budget=case["budget"])
+            ol.simple_mat(a, b, sc_ambi), (q, e, q2, e2), budget=case["budget"])
 ''' % TESTS
 
 
@@ -91,7 +94,7 @@ def _map_case(name, tmp_path):
     m = (HPC_MANIFEST if hpc else MANIFEST)[name]
     ref, reads, wfile = (make_golden.make_hpc_inputs if hpc else make_golden.make_inputs)(name, str(tmp_path))
     assert make_golden.md5(ref) == m["ref_md5"] and make_golden.md5(reads) == m["reads_md5"], "synthetic input generator drifted"
-    return dict(kind="map", name=name, ref=ref, reads=reads, w=wfile, preset=m["params"]["preset"], gap=m["params"].get("gap", [0, 0, 0, 0]),
+    return dict(kind="map", name=name, ref=ref, reads=reads, w=wfile, preset=m["params"]["preset"], scoring=make_golden.scoring_override(m["params"]),
                 hpc=int(hpc), budget=BUDGET, out=str(tmp_path / "out.paf"))
 
 
@@ -178,7 +181,8 @@ def test_crafted_dp_and_ll_match_oracle(tee_so, scoring, tmp_path):
     r = _run(tee_so, dict(kind="align", ref=str(tmp_path / "ref.fa"), scoring=scoring, budget=2 << 20), tmp_path)
     assert r.n_mismatch == 0, r.text()
     assert r["dp.scan_zdrop_jobs"] > 0 and r["dp.flag_0xc2"] > 0 and r["ll.jobs"] > 0 and r["dp.max_chunks"] >= 3
-    if scoring != "single":
+    a, b, q, e, q2, e2, sc_ambi = T.SCORINGS[scoring]
+    if (q, e) != (q2, e2):  # the single-affine sweep has no cooperative form
         assert r["dp.coop_jobs"] > 0
 
 

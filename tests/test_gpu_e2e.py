@@ -1,5 +1,6 @@
 """End-to-end parity on the GPU: PAF (coordinates, chaining/DP scores, MAPQ, CIGAR, every tag) must be
 byte-identical to the golden output of the real reference (tests/golden/, made by tools/make_golden.py)."""
+import ctypes as C
 import gzip
 import json
 import os
@@ -35,8 +36,9 @@ def test_paf_matches_reference(name, tmp_path):
     assert make_golden.md5(ref) == m["ref_md5"] and make_golden.md5(reads) == m["reads_md5"], "synthetic input generator drifted"
     exp = gzip.open(os.path.join(ROOT, "tests", "golden", name + ".paf.gz")).read()
     mp = Mapper(ref, wfile, preset=m["params"]["preset"], cigar=True)
-    if "gap" in m["params"]:  # -O4 -E2: a single gap pair, every DP call is the single-affine kernel (ksw_extz2)
-        mp.mo.q, mp.mo.e, mp.mo.q2, mp.mo.e2 = m["params"]["gap"]
+    # -O4 -E2 (a single gap pair: every DP call is the single-affine kernel, ksw_extz2) or -A / -B / --score-N / -O / -E
+    make_golden.apply_scoring(mp.mo, m["params"])
+    assert mp.L.wm_check_opt(C.byref(mp.io), C.byref(mp.mo)) == 0
     out = str(tmp_path / "out.paf")
     mp.map_file(reads, out)
     got = open(out, "rb").read()
@@ -122,10 +124,11 @@ def test_rank_sharded_outputs_merge_to_the_reference(tmp_path):
     assert multi.merge_tagged(shards) == exp
 
 
-@pytest.mark.parametrize("key,sam", [("paf_edge", False), ("sam_edge", True)])
+@pytest.mark.parametrize("key,sam", [("paf_edge", False), ("sam_edge", True), ("paf_edge_N0", False), ("paf_edge_N3", False)])
 def test_edge_case_reads_match_reference(key, sam, tmp_path):
-    """Empty, shorter-than-k, N-rich, IUPAC, lower-case, chimeric and unmappable reads (tools/make_golden.py edge_reads_of).
-    Runs in a child process: the library exits on a CUDA error, which must not take the test session with it."""
+    """Empty, shorter-than-k, N-rich, IUPAC, lower-case, chimeric and unmappable reads (tools/make_golden.py edge_reads_of),
+    also under --score-N 0 and 3.  Runs in a child process: the library exits on a CUDA error, which must not take the
+    test session with it."""
     import hashlib
     import subprocess
     name = make_golden.TAG_CASES[key][0]
@@ -133,9 +136,10 @@ def test_edge_case_reads_match_reference(key, sam, tmp_path):
     ref, reads, wfile = make_golden.make_inputs(name, str(tmp_path))
     reads = make_golden.edge_reads_of(reads, reads + ".edge.fa")
     out = str(tmp_path / "out.txt")
-    code = ("import sys; sys.path.insert(0, %r); from winnowmap_b200.mapper import Mapper; "
-            "mp = Mapper(%r, %r, preset=%r, cigar=True, sam=%r); mp.map_file(%r, %r); mp.close()"
-            % (ROOT, ref, wfile, m["params"]["preset"], sam, reads, out))
+    scoring = make_golden.TAG_CASES[key][3] if len(make_golden.TAG_CASES[key]) > 3 else None
+    code = ("import sys; sys.path[:0] = [%r, %r]; import make_golden; from winnowmap_b200.mapper import Mapper; "
+            "mp = Mapper(%r, %r, preset=%r, cigar=True, sam=%r); make_golden.apply_scoring(mp.mo, dict(scoring=%r)); mp.map_file(%r, %r); mp.close()"
+            % (ROOT, os.path.join(ROOT, "tools"), ref, wfile, m["params"]["preset"], sam, scoring, reads, out))
     subprocess.run([sys.executable, "-c", code], check=True, timeout=600)
     got = make_golden.sam_without_pg(open(out, "rb").read())
     assert hashlib.md5(got).hexdigest() == m["tag_md5"][key]

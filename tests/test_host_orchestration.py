@@ -24,16 +24,18 @@ def hostsim():
     subprocess.check_call([os.path.join(d, "build.sh")], stderr=subprocess.DEVNULL)
     L = C.CDLL(os.path.join(d, "libwm_hostsim.so"))
     L.wmt_map_file.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int]
+    L.wmt_set_scoring.argtypes = [C.c_int] * 7
     return L
 
 
-@pytest.mark.parametrize("name", ["ont_small", "hifi_small", "ont_sv", "ont_tandem", "asm20_small", "ont_single_gap"])
+@pytest.mark.parametrize("name", ["ont_small", "hifi_small", "ont_sv", "ont_tandem", "asm20_small", "ont_single_gap", "asm5_small", "asm10_small",
+                                  "ont_sv_long_inc"])
 def test_host_pipeline_matches_reference_golden(hostsim, name, tmp_path):
     m = MANIFEST[name]
     ref, reads, wfile = make_golden.make_inputs(name, str(tmp_path))
     assert make_golden.md5(ref) == m["ref_md5"] and make_golden.md5(reads) == m["reads_md5"]
     out = str(tmp_path / "o.paf")
-    hostsim.wmt_set_gap(*m["params"].get("gap", (0, 0, 0, 0)))  # -O / -E: one gap pair routes every DP call to ksw_extz2
+    hostsim.wmt_set_scoring(*make_golden.scoring_override(m["params"]))  # -A / -B / --score-N / -O / -E of the case
     rc = hostsim.wmt_map_file(ref.encode(), wfile.encode() if wfile else None, m["params"]["preset"].encode(), reads.encode(), out.encode(), 8)
     assert rc == 0
     exp = gzip.open(os.path.join(ROOT, "tests", "golden", name + ".paf.gz")).read()
@@ -73,11 +75,13 @@ def test_host_sam_writer_matches_reference_golden(hostsim, name, tmp_path):
 @pytest.mark.parametrize("key,sam,flags", [("paf_cs", 0, 0x40), ("paf_cs_long", 0, 0x40 | 0x800), ("sam_md", 1, 0x1000000),
                                             ("paf_eqx", 0, 0x4000000), ("sam_softclip", 1, 0x80000),
                                             ("sam_no2nd_hitonly", 1, 0x4000 | 0x40000000), ("paf_no_hit", 0, 0x8000000),
-                                            ("sam_fastq_comment", 1, 0x2000000), ("paf_edge", 0, 0), ("sam_edge", 1, 0)])
+                                            ("sam_fastq_comment", 1, 0x2000000), ("paf_edge", 0, 0), ("sam_edge", 1, 0),
+                                            ("paf_edge_N0", 0, 0), ("paf_edge_N3", 0, 0)])
 def test_host_output_options_match_reference(hostsim, key, sam, flags, tmp_path):
     """Output options against the reference run with the same switches: --cs / --cs=long / --MD difference strings
     (src/format.c:141-243), --eqx (=/X CIGAR, src/align.c:169-238), -Y, --secondary=no --sam-hit-only, --paf-no-hit, and
-    gzipped FASTQ input with comments under -y (QUAL column, comment copied to the record)."""
+    gzipped FASTQ input with comments under -y (QUAL column, comment copied to the record), and the N-rich edge reads
+    under --score-N 0 and 3."""
     import hashlib
     case = make_golden.TAG_CASES[key]
     name = case[0]
@@ -88,6 +92,8 @@ def test_host_output_options_match_reference(hostsim, key, sam, flags, tmp_path)
     if len(case) > 2 and case[2] == "edge":  # empty, tiny, N-rich, lower-case, chimeric, unmappable reads
         reads = make_golden.edge_reads_of(reads, reads + ".edge.fa")
     out = str(tmp_path / "o.txt")
+    if len(case) > 3:  # --score-N
+        hostsim.wmt_set_scoring(*make_golden.scoring_override(dict(scoring=case[3])))
     hostsim.wmt_map_file_flags.argtypes = [C.c_char_p] * 5 + [C.c_int, C.c_int, C.c_int64]
     rc = hostsim.wmt_map_file_flags(ref.encode(), wfile.encode() if wfile else None, m["params"]["preset"].encode(), reads.encode(), out.encode(), 8, sam, flags)
     assert rc == 0
@@ -137,3 +143,29 @@ def test_reference_packing_matches_the_plain_loop(hostsim):
             E[(o + j) >> 3] |= np.uint32(code.get(ch, 4) << (((o + j) & 7) << 2))
         o += len(sq)
     assert np.array_equal(S, E)
+
+
+def test_scorings_whose_int8_lanes_wrap_are_refused(hostsim, tmp_path):
+    """check_opt (csrc/host_io.cpp) refuses two gap pairs with -A + q + 2e > 128 (return code -7): there the reference's ksw_extd2_sse wraps its int8 lanes and the device fill, which keeps them in 16 bits,
+    would differ.  Every scoring of tee_lib.SCORINGS passes, and so do the limit itself and one gap pair (ksw_extz2 wraps
+    as the reference does).  The oracle-backed run refuses the same options."""
+    import ctypes as C
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import tee_lib as T
+    from winnowmap_b200 import lib
+    from winnowmap_b200.mapper import make_options
+
+    def check(a, b, q, e, q2, e2, sc_ambi):
+        io, mo = make_options("map-ont")
+        mo.a, mo.b, mo.q, mo.e, mo.q2, mo.e2, mo.sc_ambi = a, b, q, e, q2, e2, sc_ambi
+        return lib().wm_check_opt(C.byref(io), C.byref(mo))
+    for name, s in T.SCORINGS.items():
+        assert check(*s) == 0, name
+    assert check(*T.REFUSED_SCORINGS["wrap_probe"]) == -7
+    assert check(82, 4, 40, 3, 83, 1, 1) == 0 and check(83, 4, 40, 3, 83, 1, 1) == -7   # 82 + 40 + 6 = 128 / 129
+    assert check(121, 4, 4, 2, 24, 1, 1) == -7 and check(120, 4, 4, 2, 24, 1, 1) == 0
+    assert check(100, 4, 40, 3, 40, 3, 1) == 0                                           # one gap pair
+    m = MANIFEST["ont_small"]
+    ref, reads, wfile = make_golden.make_inputs("ont_small", str(tmp_path))
+    hostsim.wmt_set_scoring(*make_golden.scoring_override(dict(scoring=T.REFUSED_SCORINGS["wrap_probe"])))
+    assert hostsim.wmt_map_file(ref.encode(), None, m["params"]["preset"].encode(), reads.encode(), str(tmp_path / "o.paf").encode(), 8) != 0

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+import tee_lib as T
 
 
 def rand_pair(rng, tlen, err=0.1, drift=0, n_runs=0):
@@ -159,6 +160,51 @@ def test_early_out_scoring_matches_reference():
         ol.assert_ref(f"extd2_early_out:{it}", got, lambda: ol.ref_extd2(qq, tt, mat, 4, 2, 24, 1, w, 400, -1, flag))
         got = ol.oracle_extz2(qq, tt, mat, 4, 2, w, 400, -1, flag)
         ol.assert_ref(f"extz2_early_out:{it}", got, lambda: ol.ref_extz2(qq, tt, mat, 4, 2, w, 400, -1, flag))
+
+
+@pytest.mark.parametrize("name", sorted(T.SCORINGS) + sorted(T.REFUSED_SCORINGS))
+def test_every_scoring_matches_reference(name):
+    """Each scoring of tee_lib.SCORINGS (and the refused one, on which the reference's int8 lanes wrap) through the
+    oracle's ksw_extd2 (ksw_extz2 for one gap pair) and ksw_ll against the reference's functions: sizes, drifts (gaps
+    longer than long_thres), N runs in both sequences, bands, Z-drops, flags and end bonuses up to a large one."""
+    a, b, q, e, q2, e2, sc_ambi = (T.SCORINGS.get(name) or T.REFUSED_SCORINGS[name])
+    mat = ol.simple_mat(a, b, sc_ambi)
+    rng = np.random.default_rng(sum(name.encode()) + 31 * a + b)
+    for it in range(40):
+        tlen = int(rng.choice([1, 5, 17, 33, 100, 300, 700, 1500]))
+        qq, tt = rand_pair(rng, tlen, err=float(rng.choice([0.01, 0.05, 0.15])), drift=int(rng.choice([0, 0, 30, 120, 400])),
+                           n_runs=int(rng.integers(0, 3)))
+        if it % 3 == 0 and len(tt) > 20:  # N in the target as well
+            p = int(rng.integers(0, len(tt) - 10))
+            tt[p:p + int(rng.integers(1, 8))] = 4
+        w = int(rng.choice([5, 50, 200, 751, -1]))
+        zdrop = int(rng.choice([400, 200, 50, -1]))
+        end_bonus = int(rng.choice([-1, 0, 10, 1000]))
+        flag = FLAGS[it % 4] | (0x10 if it % 5 == 0 else 0)
+        if (q, e) == (q2, e2):
+            got = ol.oracle_extz2(qq, tt, mat, q, e, w, zdrop, end_bonus, flag)
+            ol.assert_ref(f"scoring:{name}:extz2:{it}", got, lambda: ol.ref_extz2(qq, tt, mat, q, e, w, zdrop, end_bonus, flag))
+        else:
+            got = ol.oracle_extd2(qq, tt, mat, q, e, q2, e2, w, zdrop, end_bonus, flag)
+            ol.assert_ref(f"scoring:{name}:extd2:{it}", got, lambda: ol.ref_extd2(qq, tt, mat, q, e, q2, e2, w, zdrop, end_bonus, flag))
+        if it % 2 == 0:
+            ol.assert_ref(f"scoring:{name}:ll:{it}", ol.oracle_ll(qq, tt, mat, q, e), lambda: ol.ref_ll(qq, tt, mat, q, e))
+
+
+def test_long_thres_of_the_scorings():
+    """long_thres / long_diff as the reference computes them (src/ksw2_extd2_sse.c:94-97) for the scorings that reach their
+    branches: asm5 ties the comparison (20, -3), long_inc takes the increment (9 -> 10), limit takes it too (20 -> 21)."""
+    def lt(q, e, q2, e2):
+        if q2 + e2 < q + e:
+            q, e, q2, e2 = q2, e2, q, e
+        t = (q2 - q) // (e - e2) - 1
+        inc = q2 + e2 + t * e2 > q + e + t * e
+        t += inc
+        return t, t * (e - e2) - (q2 - q) - e2, inc
+    assert lt(*T.SCORINGS["asm5"][2:6]) == (20, -3, False)
+    assert lt(*T.SCORINGS["long_inc"][2:6]) == (10, -2, True)
+    assert lt(*T.SCORINGS["limit"][2:6]) == (21, -2, True)
+    assert lt(*T.SCORINGS["map-ont"][2:6]) == (19, -2, False)
 
 
 @pytest.mark.parametrize("seed", range(3))

@@ -36,7 +36,34 @@ CASES = {
                            preset="map-ont", use_W=False, k=15, sv=True, extra=["-O4", "-E2"], gap=(4, 2, 4, 2)),
     "asm20_small": dict(ref_len=300000, contigs=1, tandem=True, ref_seed=1014, n_reads=12, n50=40000, err=0.02, read_seed=2014, min_len=5000,
                         preset="asm20", use_W=True, k=19, w_distinct=0.99),
+    # the other assembly presets: asm5 (gap sum 124, e - e2 = 2) and asm10
+    "asm5_small": dict(ref_len=300000, contigs=1, tandem=True, ref_seed=1015, n_reads=12, n50=40000, err=0.005, read_seed=2015, min_len=5000,
+                       preset="asm5", use_W=True, k=19, w_distinct=0.99),
+    "asm10_small": dict(ref_len=300000, contigs=1, tandem=True, ref_seed=1016, n_reads=12, n50=40000, err=0.01, read_seed=2016, min_len=5000,
+                        preset="asm10", use_W=True, k=19, w_distinct=0.99),
+    # -A2 -B5 -O4,25 -E3,1 on the structural-variant reads: long_thres is raised by one (src/ksw2_extd2_sse.c:95-96), and
+    # the long gaps of the SV reads are where the second gap pair decides.  scoring: (a, b, q, e, q2, e2, sc_ambi)
+    "ont_sv_long_inc": dict(ref_len=400000, contigs=2, tandem=False, ref_seed=1021, n_reads=60, n50=14000, err=0.04, read_seed=2021, min_len=2000,
+                            preset="map-ont", use_W=False, k=15, sv=True, extra=["-A2", "-B5", "-O4,25", "-E3,1"], scoring=(2, 5, 4, 3, 25, 1, 1)),
 }
+
+
+def scoring_override(params):
+    """The -A / -B / --score-N / -O / -E of a case as (a, b, sc_ambi, q, e, q2, e2), -1 where the preset's value stays: from
+    params["scoring"] (a, b, q, e, q2, e2, sc_ambi) or params["gap"] (q, e, q2, e2)."""
+    if params.get("scoring"):
+        a, b, q, e, q2, e2, n = params["scoring"]
+        return [a, b, n, q, e, q2, e2]
+    if params.get("gap"):
+        return [-1, -1, -1] + list(params["gap"])
+    return [-1] * 7
+
+
+def apply_scoring(mo, params):
+    """The same override on a mapping-options structure (winnowmap_b200.mapper.MapOpt)."""
+    for f, v in zip(("a", "b", "sc_ambi", "q", "e", "q2", "e2"), scoring_override(params)):
+        if v >= 0:
+            setattr(mo, f, v)
 
 
 def md5(path):
@@ -107,6 +134,10 @@ TAG_CASES = {
     "sam_fastq_comment": ("ont_small", ["-a", "-y"], "fastq"),   # gzipped FASTQ with comments: QUAL column, MM_F_COPY_COMMENT 0x2000000
     "paf_edge": ("ont_small", ["-c"], "edge"),                   # empty / tiny / N-rich / lower-case / chimeric / unmappable reads
     "sam_edge": ("ont_small", ["-a"], "edge"),
+    # the N-rich edge reads under other N scores, with the scoring as params["scoring"] has it: --score-N 0 scores N cells
+    # -e2 in the fill (src/ksw2_extd2_sse.c:79) but 0 in the alignment statistics
+    "paf_edge_N0": ("ont_small", ["-c", "--score-N", "0"], "edge", (2, 4, 4, 2, 24, 1, 0)),
+    "paf_edge_N3": ("ont_small", ["-c", "--score-N", "3"], "edge", (2, 4, 4, 2, 24, 1, 3)),
 }
 
 

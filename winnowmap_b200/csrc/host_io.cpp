@@ -99,6 +99,11 @@ int check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo)
 	if (mo->e <= 0 || mo->q <= 0) return -1;
 	if ((mo->q != mo->q2 || mo->e != mo->e2) && !(mo->e > mo->e2 && mo->q + mo->e < mo->q2 + mo->e2)) return -2;
 	if ((mo->q + mo->e) + (mo->q2 + mo->e2) > 127) return -1;
+	// Not in the reference.  With two gap pairs (q + e < q2 + e2 by the check above), ksw_extd2_sse's int8 lanes wrap once
+	// a - z + q can fall below -128 (src/ksw2_extd2_sse.c:52-58, with x, v >= -(q + e) and the score difference z <= -A),
+	// i.e. when -A + q + 2e > 128.  The device fill keeps these values in 16 bits and does not wrap, so it would silently
+	// differ from the reference: such scorings are refused.  (ksw_extz2, one gap pair, wraps as the reference does.)
+	if ((mo->q != mo->q2 || mo->e != mo->e2) && mo->a + mo->q + 2 * mo->e > 128) return -7;
 	if (mo->zdrop < mo->zdrop_inv) return -5;
 	if ((mo->flag & WM_F_NO_PRINT_2ND) && (mo->flag & WM_F_ALL_CHAINS)) return -5;
 	return 0;

@@ -2,8 +2,11 @@
 // case).  Included by ksw_extd2.cu.
 //
 // Two cells per 32-bit register as signed 16-bit halves, native 16x2 SIMD (VIADD.16x2 / VIMNMX.S16x2 /
-// VIADDMNMX.S16x2).  All DP quantities are kept multiplied by 8: the reference's int8 values (|v| <= 127 by
-// mm_check_opt, src/options.c:169) fit 16 bits without ever wrapping, and the three free low bits carry tags:
+// VIADDMNMX.S16x2).  All DP quantities are kept multiplied by 8, and the three free low bits carry tags.  The
+// reference keeps them in int8 lanes.  Those stay in [-128, 127] when the gap sum (q + e) + (q2 + e2) is at most 127
+// and -A + q + 2e at most 128 (both enforced by check_opt, csrc/host_io.cpp; the second is its return code -7, not in
+// the reference) and no score is below -2(q + e) (otherwise the fill returns before the sweep, as the reference does).
+// Times 8 that is well inside 16 bits: the sweep never wraps, and neither does the reference.  The tags:
 //  * in the max() that picks z, a tie-break tag, so that one max yields both the best state value and WHICH
 //    state produced it, in the reference's tie order (left-aligned: first of equals, src/ksw2_extd2_sse.c:227-234;
 //    right-aligned: last of equals, :274-281);
