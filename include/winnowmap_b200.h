@@ -251,6 +251,23 @@ wm_gpu_ctx *wm_index_build(const char *ref_fn, const char *kmer_freq_fn, int k, 
  * MM_I_HPC (-H, src/main.c:166) is supported; other flag bits are refused (NULL). */
 wm_gpu_ctx *wm_index_build_opt(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, int device);
 
+/* The -W list computed from the reference instead of read from a file: what `meryl count k=K ref.fa` followed by
+ * `meryl print greater-than distinct=D` lists (the recipe of the reference's README; ext/meryl/src/meryl/merylOp-nextMer.C:103-115).
+ * Canonical k-mers are counted per sequence (a k-mer never spans two sequences; any base outside ACGTacgtUu breaks it);
+ * the threshold is the first count value, ascending, at which the cumulative number of distinct k-mers reaches
+ * (uint64)(D * distinct k-mers); the list is every k-mer counted more often, ascending by code.  The codes are encodeKmer's
+ * (src/index.c:362-376).  1 <= k <= 28, 0 < D <= 1; anything else is refused (-1 / NULL).
+ * wm_topfreq returns the list's length and writes up to `cap` entries (NULL buffers with cap = 0: count only) and the
+ * threshold.  Each call counts the reference anew. */
+int64_t wm_topfreq(const char *ref_fn, int k, double distinct, uint64_t *kmers, uint32_t *counts, int64_t cap, uint64_t *threshold, int device);
+/* wm_index_build_opt with the list of wm_topfreq(ref_fn, io->k, distinct) in place of a -W file.  The reference is read
+ * once; under MM_I_HPC the list is counted on the uncompressed sequences (what meryl run on ref.fa gives), the filter
+ * is probed with the compressed k-mers as with a file. */
+wm_gpu_ctx *wm_index_build_topfreq(const char *ref_fn, const wm_idxopt_t *io, double distinct, int device);
+/* The threshold rule alone, on the host (no device needed): value[0..n) the count values that occur, ascending, occ[i]
+ * the number of distinct k-mers with count value[i].  0 for an empty histogram. */
+uint64_t wm_topfreq_threshold(const uint64_t *value, const uint64_t *occ, int64_t n, double distinct);
+
 /* One-time index fan-out (SURVEY.md 8e): the flattened index as one relocatable blob.  Rank 0 builds it, it travels
  * GPU-to-GPU in a single NCCL broadcast, every other rank re-creates its context with wm_idx_blob_load.  The index flag
  * travels in bits 16..31 of the second header word (zero without flags, so such a blob is byte-identical to before). */
@@ -328,6 +345,9 @@ int wm_device_synchronize(void);
 int wm_device_mem(double *free_bytes, double *total_bytes); /* cudaMemGetInfo of the current device */
 void wm_dump_timers(void); /* prints and resets the orchestration wall-clock accumulators (stderr) */
 
+/* n_reads, n_bases, n_minimaps, n_chained, n_dp_jobs, n_ll_jobs, n_rounds, t_seed, t_dp, t_host, t_index, t_map, n_keys,
+ * n_pos, then the -W list of wm_index_build_topfreq: its length, its threshold and the seconds spent counting it (zeros
+ * for an index built otherwise) */
 void wm_get_stats(wm_gpu_ctx *ctx, double *out, int n);
 void wm_reset_stats(wm_gpu_ctx *ctx);
 

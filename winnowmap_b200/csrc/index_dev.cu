@@ -15,8 +15,12 @@
 #define WM_IX_TILE 4096
 #define WM_IX_WARPS 4
 
-__global__ void __launch_bounds__(WM_IX_WARPS * 32)
-wm_ix_hist_kernel(const wm128_dev *__restrict__ a, int64_t n, int shift, int64_t n_tiles, int32_t *__restrict__ hist)
+// the sort key of an element: the x word of a (minimizer, position) pair, or a bare 64-bit key (csrc/topfreq.cu)
+__device__ __forceinline__ uint64_t wm_ix_key(const wm128_dev &v) { return v.x; }
+__device__ __forceinline__ uint64_t wm_ix_key(const uint64_t &v) { return v; }
+
+template <typename T> __global__ void __launch_bounds__(WM_IX_WARPS * 32)
+wm_ix_hist_kernel(const T *__restrict__ a, int64_t n, int shift, int64_t n_tiles, int32_t *__restrict__ hist)
 {
 	__shared__ int cnt[WM_IX_WARPS][256];
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -25,14 +29,14 @@ wm_ix_hist_kernel(const wm128_dev *__restrict__ a, int64_t n, int shift, int64_t
 	__syncwarp();
 	if (tile < n_tiles) {
 		const int64_t beg = tile * WM_IX_TILE, end = beg + WM_IX_TILE < n ? beg + WM_IX_TILE : n;
-		for (int64_t i = beg + lane; i < end; i += 32) atomicAdd(&cnt[wid][(int)(a[i].x >> shift & 255)], 1);
+		for (int64_t i = beg + lane; i < end; i += 32) atomicAdd(&cnt[wid][(int)(wm_ix_key(a[i]) >> shift & 255)], 1);
 		__syncwarp();
 		for (int d = lane; d < 256; d += 32) hist[(int64_t)d * n_tiles + tile] = cnt[wid][d]; // digit-major: one scan gives every tile's bases
 	}
 }
 
-__global__ void __launch_bounds__(WM_IX_WARPS * 32)
-wm_ix_scatter_kernel(const wm128_dev *__restrict__ a, wm128_dev *__restrict__ b, int64_t n, int shift, int64_t n_tiles, const int64_t *__restrict__ offs)
+template <typename T> __global__ void __launch_bounds__(WM_IX_WARPS * 32)
+wm_ix_scatter_kernel(const T *__restrict__ a, T *__restrict__ b, int64_t n, int shift, int64_t n_tiles, const int64_t *__restrict__ offs)
 {
 	__shared__ long long base[WM_IX_WARPS][256];
 	const unsigned FULL = 0xffffffffu;
@@ -45,9 +49,9 @@ wm_ix_scatter_kernel(const wm128_dev *__restrict__ a, wm128_dev *__restrict__ b,
 	const unsigned lt = (1u << lane) - 1u;
 	for (int64_t i0 = beg; i0 < end; i0 += 32) {
 		const int64_t i = i0 + lane;
-		wm128_dev v; v.x = v.y = 0;
+		T v = {};
 		int d = -1 - lane; // lanes past the end match nobody
-		if (i < end) { v = a[i]; d = (int)(v.x >> shift & 255); }
+		if (i < end) { v = a[i]; d = (int)(wm_ix_key(v) >> shift & 255); }
 		const unsigned m = __match_any_sync(FULL, d);
 		long long dst = 0;
 		if (i < end) dst = base[wid][d] + __popc(m & lt);
@@ -75,31 +79,39 @@ __global__ void wm_ix_csr_kernel(const wm128_dev *__restrict__ a, int64_t n, con
 	if (flag[i]) { const int64_t k = key_idx[i]; keys[k] = a[i].x >> 8; pos_off[k] = (uint64_t)i; }
 }
 
+// Stable LSD radix sort of the n elements of a by key bits [bit_lo, bit_hi), 8 bits per pass, ping-pong between a and b.
+// Returns the buffer that holds the result.
+template <typename T> T *wm_lsd_sort(T *a, T *b, int64_t n, int bit_lo, int bit_hi, cudaStream_t st)
+{
+	if (n <= 0 || bit_lo >= bit_hi) return a;
+	T *bufs[2] = { a, b };
+	const int64_t n_tiles = (n + WM_IX_TILE - 1) / WM_IX_TILE;
+	int cur = 0;
+	int32_t *d_hist = wm_dev_alloc<int32_t>(256 * n_tiles + 1);
+	int64_t *d_offs = wm_dev_alloc<int64_t>(256 * n_tiles + 2);
+	int64_t *d_tmp = wm_dev_alloc<int64_t>(wm_scan_tmp_elems(256 * n_tiles) + 1);
+	const unsigned grid = (unsigned)((n_tiles + WM_IX_WARPS - 1) / WM_IX_WARPS);
+	for (int shift = bit_lo; shift < bit_hi; shift += 8) {
+		wm_count_launch(); wm_ix_hist_kernel<T><<<grid, WM_IX_WARPS * 32, 0, st>>>(bufs[cur], n, shift, n_tiles, d_hist);
+		wm_exclusive_scan(d_hist, 256 * n_tiles, d_offs, d_tmp, st);
+		wm_count_launch(); wm_ix_scatter_kernel<T><<<grid, WM_IX_WARPS * 32, 0, st>>>(bufs[cur], bufs[cur ^ 1], n, shift, n_tiles, d_offs);
+		WM_CUDA_CHECK(cudaGetLastError());
+		cur ^= 1;
+	}
+	WM_CUDA_CHECK(cudaStreamSynchronize(st));
+	cudaFree(d_hist); cudaFree(d_offs); cudaFree(d_tmp);
+	return bufs[cur];
+}
+template uint64_t *wm_lsd_sort<uint64_t>(uint64_t *, uint64_t *, int64_t, int, int, cudaStream_t);
+
 // d_a: n pairs in position order (consumed: used as one of the two sort buffers and freed).  k: the k-mer length (the hash has
 // 2k significant bits, src/sketch.c:150).  On return the three CSR arrays are device allocations owned by the caller.
 void wm_index_build_dev(wm128_dev *d_a, int64_t n, int k, uint64_t **d_keys_out, uint64_t **d_pos_off_out, uint64_t **d_pos_out, int64_t *n_keys_out, cudaStream_t st)
 {
 	wm128_dev *bufs[2] = { d_a, wm_dev_alloc<wm128_dev>(n + 1) };
-	const int64_t n_tiles = (n + WM_IX_TILE - 1) / WM_IX_TILE;
-	int cur = 0;
-	if (n > 0) {
-		int32_t *d_hist = wm_dev_alloc<int32_t>(256 * n_tiles + 1);
-		int64_t *d_offs = wm_dev_alloc<int64_t>(256 * n_tiles + 2);
-		int64_t *d_tmp = wm_dev_alloc<int64_t>(wm_scan_tmp_elems(256 * n_tiles) + 1);
-		const unsigned grid = (unsigned)((n_tiles + WM_IX_WARPS - 1) / WM_IX_WARPS);
-		const int key_bits = 2 * k < 56 ? 2 * k : 56;
-		for (int bit = 0; bit < key_bits; bit += 8) {
-			const int shift = 8 + bit; // the hash sits above the 8-bit span in x (src/sketch.c:122)
-			wm_count_launch(); wm_ix_hist_kernel<<<grid, WM_IX_WARPS * 32, 0, st>>>(bufs[cur], n, shift, n_tiles, d_hist);
-			wm_exclusive_scan(d_hist, 256 * n_tiles, d_offs, d_tmp, st);
-			wm_count_launch(); wm_ix_scatter_kernel<<<grid, WM_IX_WARPS * 32, 0, st>>>(bufs[cur], bufs[cur ^ 1], n, shift, n_tiles, d_offs);
-			WM_CUDA_CHECK(cudaGetLastError());
-			cur ^= 1;
-		}
-		WM_CUDA_CHECK(cudaStreamSynchronize(st));
-		cudaFree(d_hist); cudaFree(d_offs); cudaFree(d_tmp);
-	}
-	const wm128_dev *s = bufs[cur];
+	const int key_bits = 2 * k < 56 ? 2 * k : 56;
+	// the hash sits above the 8-bit span in x (src/sketch.c:122)
+	const wm128_dev *s = wm_lsd_sort(bufs[0], bufs[1], n, 8, 8 + key_bits, st);
 	// CSR: key boundaries -> key index (prefix sum) -> keys / pos_off / pos
 	int32_t *d_flag = wm_dev_alloc<int32_t>(n + 1);
 	int64_t *d_kidx = wm_dev_alloc<int64_t>(n + 2);

@@ -33,7 +33,7 @@ F_NO_DIAG, F_NO_DUAL, F_NO_LJOIN, F_FOR_ONLY, F_REV_ONLY, F_ALL_CHAINS = 0x001, 
 I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
 
 STAT_NAMES = ("n_reads", "n_bases", "n_minimaps", "n_chained", "n_dp_jobs", "n_ll_jobs", "n_rounds", "t_seed", "t_dp", "t_host",
-              "t_index", "t_map", "n_keys", "n_pos")
+              "t_index", "t_map", "n_keys", "n_pos", "n_topfreq", "topfreq_threshold", "t_topfreq")
 
 
 def _setup(L):
@@ -45,6 +45,12 @@ def _setup(L):
     L.wm_index_build.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int]
     L.wm_index_build_opt.restype = C.c_void_p
     L.wm_index_build_opt.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(IdxOpt), C.c_int]
+    L.wm_index_build_topfreq.restype = C.c_void_p
+    L.wm_index_build_topfreq.argtypes = [C.c_char_p, C.POINTER(IdxOpt), C.c_double, C.c_int]
+    L.wm_topfreq.restype = C.c_int64
+    L.wm_topfreq.argtypes = [C.c_char_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64), C.c_int]
+    L.wm_topfreq_threshold.restype = C.c_uint64
+    L.wm_topfreq_threshold.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_double]
     L.wm_idx_flag.argtypes = [C.c_void_p]
     L.wm_gpu_destroy.argtypes = [C.c_void_p]
     L.wm_idx_blob_size.restype = C.c_int64
@@ -96,10 +102,17 @@ class Mapper:
     """winnowmap [-W rep.txt] -x preset [-H] -c ref.fa reads.fa  on one GPU.  hpc=True is -H: the index and the reads are
     sketched with homopolymer-compressed k-mers (reference src/main.c:166).  A blob carries its own flag.  no_diag, dual,
     all_vs_all and strand are the self / all-vs-all and single-strand options of make_options (-D, --dual, -X,
-    --for-only / --rev-only): Mapper(reads, preset="map-ont", all_vs_all=True).map_file(reads, out) computes overlaps."""
+    --for-only / --rev-only): Mapper(reads, preset="map-ont", all_vs_all=True).map_file(reads, out) computes overlaps.
+    distinct=D takes the -W list from the reference itself instead of the file kmer_freq: the k-mers that
+    `meryl count k=K` + `meryl print greater-than distinct=D` list (top_kmers), counted on the GPU; 0.9998 is the
+    reference README's recipe."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
-                 no_diag=False, dual=True, all_vs_all=False, strand=None):
+                 no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None):
+        if kmer_freq is not None and distinct is not None:
+            raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
+        if distinct is not None and not 0.0 < distinct <= 1.0:
+            raise ValueError(f"distinct must be in (0, 1], not {distinct!r}")
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand)
         if hpc:
@@ -108,6 +121,8 @@ class Mapper:
         if blob is not None:  # index received from another rank (numpy uint8 array)
             self._blob_keep = blob
             self.ctx = self.L.wm_idx_blob_load(blob.ctypes.data, blob.nbytes, device)
+        elif distinct is not None:
+            self.ctx = self.L.wm_index_build_topfreq(ref.encode(), C.byref(self.io), float(distinct), device)
         else:
             self.ctx = self.L.wm_index_build_opt(ref.encode(), kmer_freq.encode() if kmer_freq else None, C.byref(self.io), device)
         if not self.ctx:
@@ -149,3 +164,33 @@ class Mapper:
             self.close()
         except Exception:
             pass
+
+
+def top_kmers(ref, k, distinct=0.9998, device=0):
+    """(kmers, counts, threshold) of `meryl count k=K ref` + `meryl print greater-than distinct=D`, counted on the GPU:
+    canonical k-mer codes (encodeKmer's, reference src/index.c:362-376) ascending as uint64, their counts as uint32, and the
+    count they are all above."""
+    import numpy as np
+    L = _setup(lib())
+    if not 1 <= k <= 28 or not 0.0 < distinct <= 1.0:
+        raise ValueError(f"k = {k} must be in 1..28 and distinct = {distinct} in (0, 1]")
+    thr = C.c_uint64(0)
+    n = L.wm_topfreq(ref.encode(), k, float(distinct), None, None, 0, C.byref(thr), device)
+    if n < 0:
+        raise RuntimeError("wm_topfreq failed")
+    kmers, counts = np.zeros(n, dtype=np.uint64), np.zeros(n, dtype=np.uint32)
+    if n:
+        m = L.wm_topfreq(ref.encode(), k, float(distinct), kmers.ctypes.data, counts.ctypes.data, n, C.byref(thr), device)
+        assert m == n, (m, n)
+    return kmers, counts, int(thr.value)
+
+
+def write_top_kmers(ref, out, k, distinct=0.9998, device=0):
+    """The -W file of top_kmers: one `KMER<TAB>COUNT` line per k-mer, spelled from its code (the format the reference reads,
+    src/index.c:390-432).  Returns (number of k-mers, threshold)."""
+    kmers, counts, thr = top_kmers(ref, k, distinct, device)
+    shifts = [2 * (k - 1 - i) for i in range(k)]
+    with open(out, "w") as f:
+        for v, c in zip(kmers.tolist(), counts.tolist()):
+            f.write("".join("ACGT"[(v >> s) & 3] for s in shifts) + f"\t{c}\n")
+    return len(kmers), thr
