@@ -264,6 +264,35 @@ int64_t wm_topfreq(const char *ref_fn, int k, double distinct, uint64_t *kmers, 
  * once; under MM_I_HPC the list is counted on the uncompressed sequences (what meryl run on ref.fa gives), the filter
  * is probed with the compressed k-mers as with a file. */
 wm_gpu_ctx *wm_index_build_topfreq(const char *ref_fn, const wm_idxopt_t *io, double distinct, int device);
+/* A multi-part index, as the reference builds it when the reference is longer than -I (mm_idx_reader_read in the loop of
+ * src/main.c:384; mm_idx_gen, src/index.c:289-297, :668-671): parts of about io->batch_size bases, read in mini-batches of
+ * min(io->mini_batch_size, io->batch_size) bases of whole sequences, and no further mini-batch once a part holds more than
+ * batch_size bases (a cumulative length equal to batch_size does not end a part; a sequence is never split; rid restarts at
+ * 0 in every part).  The FASTA is read, the -W list (kmer_freq_fn, or with distinct > 0 counted over the whole reference as
+ * wm_index_build_topfreq does) and its filter built once; each part is sketched, sorted and hashed on the device and all
+ * parts stay resident.  The parts share one set of lanes (streams, workspaces, DP budget).  A reference that fits one part
+ * gives an ordinary single index.  wm_index_build / _opt / _topfreq always build one index whatever the size.
+ * On a multi-part context: wm_map_file writes part-major (one pass per part), or merged under opt->split_prefix;
+ * wm_gpu_map_batch returns the merged hits under split_prefix (rep_len and frag_gap 0, as the reference's merge pass leaves
+ * them) and is refused otherwise; the wm_idx_n_seq / seq_name / seq_len / name2id accessors see all parts' sequences in
+ * part order; wm_idx_getseq, wm_gen_cs / _MD, wm_idx_cal_max_occ, the blob calls and wm_bench_upload are refused. */
+wm_gpu_ctx *wm_index_build_parts(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, double distinct, int device);
+/* the number of parts (1 for every other context) and part i, a borrowed context (NULL out of range; the context itself
+ * for i = 0 of a single index) usable with wm_gpu_map_batch, wm_map, wm_map_file and the wm_idx_* accessors; the parts of one
+ * context map one call at a time; wm_gpu_destroy of a part does nothing, the whole index goes with its root */
+int wm_idx_n_parts(const wm_gpu_ctx *ctx);
+wm_gpu_ctx *wm_idx_part(wm_gpu_ctx *ctx, int i);
+/* the part plan of wm_index_build_parts on the host (no device needed): the number of sequences of each part into
+ * n_seq[0..cap); returns the number of parts, -1 if the file cannot be read */
+int wm_part_plan(const char *ref_fn, uint64_t batch_size, int mini_batch_size, int32_t *n_seq, int cap);
+/* mm_idx_cal_max_occ (src/index.c:173-194) of one index: INT32_MAX for f <= 0, else the ((1 - f) * n)-th smallest occurrence
+ * count over its n keys (a singleton counts 1) plus one, selected on the device from the CSR offsets and remembered per f.
+ * -1 with a message where the reference would read past its array (the rank reaches n) and on a multi-part context. */
+int32_t wm_idx_cal_max_occ(const wm_gpu_ctx *ctx, float f);
+/* mm_mapopt_update (src/options.c:71-81) against one index: MM_F_SPLICE from the splice strand flags, mid_occ from
+ * mid_occ_frac when 0 <= f < 1, then at least min_mid_occ.  0, or -1 when wm_idx_cal_max_occ refuses.  wm_map_file and
+ * wm_gpu_map_batch apply it per part themselves when mid_occ_frac is set (-f), so a caller need not. */
+int wm_mapopt_update(wm_mapopt_t *opt, const wm_gpu_ctx *ctx);
 /* The threshold rule alone, on the host (no device needed): value[0..n) the count values that occur, ascending, occ[i]
  * the number of distinct k-mers with count value[i].  0 for an empty histogram. */
 uint64_t wm_topfreq_threshold(const uint64_t *value, const uint64_t *occ, int64_t n, double distinct);

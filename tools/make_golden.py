@@ -483,10 +483,203 @@ def main_overlap():
     json.dump(manifest, open(os.path.join(gdir, "overlap_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- index parts (-I), --split-prefix and -f: tests/golden/parts_manifest.json and parts_*; the other manifests are not touched ----
+# "multi": six contigs of unequal length with tandem arrays and ONT reads, -W from the stand-in list; -I 330k cuts it into
+# three parts.  Plan inputs: FASTA files whose part boundaries sit on the rules' edges, mapped with one read so that the
+# reference prints its per-part sequence counts.
+MULTI = dict(ref_len=900000, ref_seed=1041, n_reads=50, n50=9000, err=0.05, read_seed=2041, min_len=1000, k=15)
+PLAN_CASES = {
+    # name: (contig lengths or ("random", n, lo, hi, seed), -I)
+    "plan_many_small": (("random", 300, 50, 4000, 5), 60000),
+    "plan_equal_I": ([1000] * 12, 3000),            # a mini-batch of exactly -I bases does not end the part
+    "plan_long_contig": ([500, 20000, 700, 800, 9000, 300], 5000),
+    "plan_zero_len": ([3000, 0, 2000, 0, 0, 4000, 0, 1000, 0], 2500),
+    "plan_I_above_ref": (("random", 40, 100, 2000, 6), 1000000000),
+}
+PARTS_CASES = {
+    # name: (inputs, reference options, library options of Mapper)
+    "parts_ont_c": ("multi", ["-x", "map-ont", "-c", "-I", "330k"], dict(preset="map-ont", part_bases=330000)),
+    "parts_ont_c_split": ("multi", ["-x", "map-ont", "-c", "-I", "330k", "--split-prefix", "SPLIT"], dict(preset="map-ont", part_bases=330000, split=True)),
+    "parts_ont_a": ("multi", ["-x", "map-ont", "-a", "-I", "330k"], dict(preset="map-ont", sam=True, part_bases=330000)),
+    "parts_ont_a_split": ("multi", ["-x", "map-ont", "-a", "-I", "330k", "--split-prefix", "SPLIT"],
+                          dict(preset="map-ont", sam=True, part_bases=330000, split=True)),
+    "parts_single_split_a": ("multi", ["-x", "map-ont", "-a", "--split-prefix", "SPLIT"], dict(preset="map-ont", sam=True, split=True)),
+    "parts_single_split_c": ("multi", ["-x", "map-ont", "-c", "--split-prefix", "SPLIT"], dict(preset="map-ont", split=True)),
+    "parts_hpc_c": ("multi", ["-x", "map-ont", "-H", "-c", "-I", "330k"], dict(preset="map-ont", hpc=True, part_bases=330000)),
+    "parts_ava_X_split": ("ava", ["-x", "map-ont", "-X", "-I", "120k", "--split-prefix", "SPLIT"],
+                          dict(preset="map-ont", cigar=False, all_vs_all=True, part_bases=120000, split=True)),
+    "parts_tandem_f0002": ("tandem", ["-x", "map-ont", "-c", "-f", "0.0002"], dict(preset="map-ont", mid_occ_frac=0.0002)),
+    "parts_tandem_f01": ("tandem", ["-x", "map-ont", "-c", "-f", "0.01"], dict(preset="map-ont", mid_occ_frac=0.01)),
+    "parts_tandem_f0002_I": ("tandem", ["-x", "map-ont", "-c", "-f", "0.0002", "-I", "199999"],
+                             dict(preset="map-ont", mid_occ_frac=0.0002, part_bases=199999)),
+    "parts_tandem_f01_I_split": ("tandem", ["-x", "map-ont", "-c", "-f", "0.01", "-I", "199999", "--split-prefix", "SPLIT"],
+                                 dict(preset="map-ont", mid_occ_frac=0.01, part_bases=199999, split=True)),
+}
+
+
+def make_multi_inputs(outdir):
+    """Six contigs of unequal length (tandem arrays in each), ONT-like reads and the stand-in -W list."""
+    c = MULTI
+    os.makedirs(outdir, exist_ok=True)
+    ref, reads, wfile = (os.path.join(outdir, "parts_multi" + x) for x in (".ref.fa", ".reads.fa", ".rep.txt"))
+    rng = np.random.default_rng(c["ref_seed"])
+    lens = [90000, 210000, 60000, 240000, 120000, 180000]
+    contigs = []
+    for i, L in enumerate(lens):
+        (_, seq), = gen_data.make_ref(rng, L, 1, True)
+        contigs.append((f"ctg{i + 1}", seq))
+    gen_data.write_fasta(ref, contigs)
+    recs = gen_data.make_reads(np.random.default_rng(c["read_seed"]), contigs, c["n_reads"], c["n50"], c["err"], min_len=c["min_len"])
+    gen_data.write_fasta(reads, recs)
+    gen_data.write_top_kmers(wfile, contigs, c["k"], 0.9998)
+    return ref, reads, wfile
+
+
+def make_parts_inputs(inputs, outdir):
+    """(index FASTA, reads FASTA, -W file or None) of one parts input set."""
+    if inputs == "multi":
+        return make_multi_inputs(outdir)
+    if inputs == "ava":
+        return make_overlap_inputs("ava", outdir)
+    return make_inputs("ont_tandem", outdir)
+
+
+def make_plan_input(name, outdir):
+    """The FASTA of a plan case (sequence names s0, s1, ...; zero-length sequences are empty records)."""
+    spec, _ = PLAN_CASES[name]
+    if isinstance(spec, tuple):
+        _, n, lo, hi, seed = spec
+        spec = [int(x) for x in np.random.default_rng(seed).integers(lo, hi + 1, n)]
+    rng = np.random.default_rng(len(spec))
+    os.makedirs(outdir, exist_ok=True)
+    fn = os.path.join(outdir, name + ".fa")
+    gen_data.write_fasta(fn, [(f"s{i}", gen_data.random_seq(rng, L)) for i, L in enumerate(spec)])
+    return fn
+
+
+def ref_part_log(err):
+    """(per-part sequence counts, per-part mid_occ) from the reference's stderr."""
+    import re
+    n_seq = [int(x) for x in re.findall(rb"loaded/built the index for (\d+) target sequence", err)]
+    mid = [int(x) for x in re.findall(rb"mid-occ:(\d+)", err)]
+    return n_seq, mid
+
+
+def main_parts():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_parts"
+    os.makedirs(tmp, exist_ok=True)
+    manifest = {"plan": {}, "cases": {}}
+    one_read = os.path.join(tmp, "one_read.fa")
+    gen_data.write_fasta(one_read, [("r0", gen_data.random_seq(np.random.default_rng(3), 3000))])
+    for name, (_, I) in PLAN_CASES.items():
+        fa = make_plan_input(name, tmp)
+        err = subprocess.run([refbin, "-t", "1", "-x", "map-ont", "-I", str(I), fa, one_read], stdout=subprocess.PIPE,
+                             stderr=subprocess.PIPE, check=True).stderr
+        n_seq, _ = ref_part_log(err)
+        manifest["plan"][name] = dict(I=I, fa_md5=md5(fa), n_seq=n_seq)
+        print(name, n_seq)
+    for name, (inputs, args, lib_opts) in PARTS_CASES.items():
+        ref, reads, wfile = make_parts_inputs(inputs, tmp)
+        args = [a if a != "SPLIT" else os.path.join(tmp, name + ".split") for a in args]
+        cmd = [refbin, "-t", "4"] + args + (["-W", wfile] if wfile else []) + [ref, reads]
+        p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True)
+        out = p.stdout
+        n_seq, mid = ref_part_log(p.stderr)
+        m = dict(inputs=inputs, lib=lib_opts, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile) if wfile else None,
+                 cmd=" ".join(["winnowmap"] + [a if not a.startswith(tmp) else "<prefix>" for a in cmd[1:-2]] + ["ref.fa", "reads.fa"]),
+                 n_seq=n_seq, mid_occ=mid)
+        if lib_opts.get("sam"):
+            body = sam_without_pg(out)
+            with gzip.GzipFile(os.path.join(gdir, name + ".sam.stripped.gz"), "wb", mtime=0) as f:
+                f.write(sam_strip_seq(body))
+            m["sam_md5"], m["n_lines"] = hashlib.md5(body).hexdigest(), body.count(b"\n")
+        else:
+            with gzip.GzipFile(os.path.join(gdir, name + ".paf.gz"), "wb", mtime=0) as f:
+                f.write(out)
+            m["paf_md5"], m["n_lines"] = hashlib.md5(out).hexdigest(), out.count(b"\n")
+        manifest["cases"][name] = m
+        print(name, m["n_lines"], "lines, parts", n_seq, "mid_occ", mid)
+    manifest["occ"] = record_occ(tmp)
+    json.dump(manifest, open(os.path.join(gdir, "parts_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
+# -f values whose mm_idx_cal_max_occ the reference computes on each part of every parts input (the tiny one is refused)
+OCC_F = [0.0, 0.0002, 0.001, 0.01, 0.1, 0.5, 0.9]
+
+
+_ref_parts = []
+
+
+def ref_parts_lib():
+    """oracle/ref_harness_parts.cpp compiled (once per process, into a temporary directory) against the reference built by
+    oracle/build_ref.sh; None where the reference's sources ($REF, default /root/reference) or that build are absent."""
+    import ctypes as C
+    import tempfile
+    if not _ref_parts:
+        src = os.path.join(os.environ.get("REF", "/root/reference"), "src")
+        lib_a = os.path.join(ROOT, "oracle", "_ref", "libwinnowmap.a")
+        so = None
+        if os.path.isdir(src) and os.path.exists(lib_a):
+            so = os.path.join(tempfile.mkdtemp(prefix="wm_ref_parts_"), "libref_harness_parts.so")
+            subprocess.check_call(["/usr/bin/g++", "-O2", "-fopenmp", "-std=c++11", "-w", "-fPIC", "-shared", "-DHAVE_KALLOC", "-I" + src,
+                                   os.path.join(ROOT, "oracle", "ref_harness_parts.cpp"), lib_a, "-o", so, "-lm", "-lz", "-lpthread"])
+        _ref_parts.append(C.CDLL(so) if so else None)
+    return _ref_parts[0]
+
+
+def ref_parts(ref, wfile, k, w, flag, batch_size):
+    """The reference's index parts of a FASTA: [(n_seq, occurrence counts as uint32, {f: mm_idx_cal_max_occ})]."""
+    import ctypes as C
+    R = ref_parts_lib()
+    assert R is not None, "the reference's sources and oracle/_ref (oracle/build_ref.sh) are needed"
+    R.ref_idx_reader_open.restype = C.c_void_p
+    R.ref_idx_reader_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_uint64]
+    R.ref_idx_reader_next.restype = C.c_void_p
+    R.ref_idx_reader_next.argtypes = [C.c_void_p, C.c_char_p]
+    R.ref_idx_reader_close.argtypes = [C.c_void_p]
+    R.ref_idx_part_n_seq.argtypes = [C.c_void_p]
+    R.ref_idx_part_counts.restype = C.c_int64
+    R.ref_idx_part_counts.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    R.ref_idx_cal_max_occ.restype = C.c_int32
+    R.ref_idx_cal_max_occ.argtypes = [C.c_void_p, C.c_float]
+    R.ref_idx_part_free.argtypes = [C.c_void_p]
+    r = R.ref_idx_reader_open(ref.encode(), w, k, flag, batch_size)
+    out = []
+    while True:
+        mi = R.ref_idx_reader_next(r, wfile.encode() if wfile else None)
+        if not mi:
+            break
+        n = R.ref_idx_part_counts(mi, None, 0)
+        cnt = np.zeros(n, np.uint32)
+        R.ref_idx_part_counts(mi, cnt.ctypes.data, n)
+        out.append((R.ref_idx_part_n_seq(mi), cnt, {f: int(R.ref_idx_cal_max_occ(mi, f)) for f in OCC_F}))
+        R.ref_idx_part_free(mi)
+    R.ref_idx_reader_close(r)
+    return out
+
+
+def record_occ(tmp):
+    """Per parts input and -I: each part's count histogram ({count: keys}) and the reference's mm_idx_cal_max_occ."""
+    rec = {}
+    for inputs, I, flag in (("multi", 330000, 0), ("multi", 330000, 1), ("tandem", 199999, 0), ("tandem", 4000000000, 0), ("ava", 120000, 0)):
+        ref, _, wfile = make_parts_inputs(inputs, tmp)
+        parts = ref_parts(ref, wfile, 15, 50, flag, I)
+        rec[f"{inputs}_I{I}_flag{flag}"] = dict(inputs=inputs, I=I, flag=flag, k=15, w=50, parts=[
+            dict(n_seq=n, hist={str(v): int(c) for v, c in zip(*np.unique(cnt, return_counts=True))}, max_occ={str(f): v for f, v in occ.items()})
+            for n, cnt, occ in parts])
+    return rec
+
+
 if __name__ == "__main__":
     if "--hpc" in sys.argv:
         main_hpc()
     elif "--overlap" in sys.argv:
         main_overlap()
+    elif "--parts" in sys.argv:
+        main_parts()
     else:
         main()

@@ -15,10 +15,12 @@
 #include "sketch.cuh"
 #include "index_dev.cuh"
 #include "topfreq.cuh"
+#include "occ_select.cuh"
 #include "gpu_backend.h"
 #include "host_io.h"
 #include "host_index.h"
 #include "host_timers.h"
+#include "host_glue.h"
 
 using namespace wmh;
 
@@ -40,7 +42,16 @@ struct wm_gpu_ctx_s {
 	std::vector<uint64_t> keys, pos_off, pos;
 	std::vector<uint8_t> bloom;
 	uint64_t bloom_bits;
+	// A multi-part index (wm_index_build_parts): the root owns the parts and the lanes, and its hidx is the sequence table
+	// of all parts (names and lengths, no sequence); be is parts[0]->be.  A part is a borrowed context whose root is set:
+	// it maps with the root's lanes, bound to its own index arrays.
+	std::vector<wm_gpu_ctx_s*> parts;
+	wm_gpu_ctx_s *root = 0;
+	std::mutex occ_mu; std::vector<std::pair<float, int32_t>> occ_cache; // mid_occ of each mid_occ_frac asked for (wm_idx_cal_max_occ)
 };
+
+static bool is_multi(const wm_gpu_ctx_s *c) { return c->parts.size() > 1; }
+static wm_gpu_ctx_s *root_of(wm_gpu_ctx_s *c) { return c->root ? c->root : c; }
 
 static void free_reg_vectors(std::vector<std::vector<wm_reg1_t>> &regs);
 static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -80,7 +91,11 @@ static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector
                       std::vector<int> &rl, std::vector<int> &fg, int n_threads, bool resident)
 {
 	(void)resident;
-	ensure_lanes(c, n_threads);
+	wm_gpu_ctx_s *r = root_of(c);
+	ensure_lanes(r, n_threads);
+	for (Backend *lane : r->lanes) gpu_backend_bind(lane, c->be); // a part of a multi-part index maps with the root's lanes
+	MapStats &stats = r->stats;
+	const std::vector<Backend*> &lanes = r->lanes;
 	const int n = (int)reads.size();
 	regs.assign(n, std::vector<wm_reg1_t>()); rl.assign(n, 0); fg.assign(n, 0);
 	if (n == 0) return;
@@ -93,14 +108,14 @@ static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector
 		const char *e = getenv("WM_CHUNK_BASES");
 		int64_t total = 0, acc = 0;
 		for (int i = 0; i < n; ++i) total += (int64_t)reads[i]->seq.size();
-		int64_t chunk_bases = total / (2 * (int64_t)c->lanes.size()) + 1;
+		int64_t chunk_bases = total / (2 * (int64_t)lanes.size()) + 1;
 		if (chunk_bases < 4000000) chunk_bases = 4000000;
 		if (chunk_bases > 16000000) chunk_bases = 16000000; // eight lanes' workspaces for chunks of this size fit an 80 GB H100
 		if (e && atoll(e) > 0) chunk_bases = atoll(e);
 		// whole rounds: the latency of a chunk grows much more slowly than its size (it is set by the serial giant tasks of
 		// its waves), so a lone chunk left over after the last full round costs almost a whole round.  The chunk size is
 		// therefore adjusted (up to +35 %) so that the chunks fill a whole number of rounds of the lanes.
-		const int64_t n_lanes = (int64_t)c->lanes.size();
+		const int64_t n_lanes = (int64_t)lanes.size();
 		int64_t rounds = (int64_t)((double)total / (double)(n_lanes * chunk_bases) + 0.35);
 		if (rounds < 1) rounds = 1;
 		if (total > n_lanes * chunk_bases * 13 / 20) chunk_bases = (total + n_lanes * rounds - 1) / (n_lanes * rounds);
@@ -111,10 +126,10 @@ static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector
 		}
 	}
 	const int n_chunks = (int)cb.size() - 1;
-	int L = (int)c->lanes.size();
+	int L = (int)lanes.size();
 	if (L > n_chunks) L = n_chunks;
 	if (L == 1 && n_chunks == 1) {
-		map_batch(c->lanes[0], &c->hidx, opt, reads, regs, rl, fg, n_threads, &c->stats);
+		map_batch(lanes[0], &c->hidx, opt, reads, regs, rl, fg, n_threads, &stats);
 		wm_dbuf_async = false; // the caller's thread may go on to the one-shot kernel entry points, which allocate synchronously
 		return;
 	}
@@ -132,7 +147,7 @@ static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector
 				std::vector<const wm_read*> sub(reads.begin() + cb[j], reads.begin() + cb[j + 1]);
 				std::vector<std::vector<wm_reg1_t>> r2; std::vector<int> rl2, fg2;
 				const double tb0 = wmh::Timers::now();
-				map_batch(c->lanes[l], &c->hidx, opt, sub, r2, rl2, fg2, thr, &st[l]);
+				map_batch(lanes[l], &c->hidx, opt, sub, r2, rl2, fg2, thr, &st[l]);
 				wmh::g_timers.add("lane.map_batch", wmh::Timers::now() - tb0);
 				for (size_t k = 0; k < sub.size(); ++k) { const int i = cb[j] + (int)k; regs[i].swap(r2[k]); rl[i] = rl2[k]; fg[i] = fg2[k]; }
 			}
@@ -145,7 +160,7 @@ static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector
 		for (int l = 0; l < L; ++l) wmh::g_timers.add("lane.idle_tail", t_end - lane_end[l]);
 	}
 	for (int l = 0; l < L; ++l) {
-		MapStats &a = c->stats; const MapStats &b = st[l];
+		MapStats &a = stats; const MapStats &b = st[l];
 		a.n_reads += b.n_reads, a.n_bases += b.n_bases, a.n_minimaps += b.n_minimaps, a.n_chained += b.n_chained, a.n_dp_jobs += b.n_dp_jobs;
 		a.n_ll_jobs += b.n_ll_jobs, a.n_rounds += b.n_rounds, a.t_seed += b.t_seed, a.t_dp += b.t_dp, a.t_host += b.t_host;
 	}
@@ -197,9 +212,11 @@ extern "C" int wm_idx_flag(const wm_gpu_ctx_s *c) { return c->hidx.flag; }
 
 extern "C" void wm_gpu_destroy(wm_gpu_ctx_s *c)
 {
-	if (!c) return;
+	if (!c || c->root) return; // a part belongs to its root
 	for (size_t i = 1; i < c->lanes.size(); ++i) gpu_backend_destroy(c->lanes[i]); // clones first: they borrow the owner's index
-	gpu_backend_destroy(c->be);
+	if (is_multi(c)) {
+		for (wm_gpu_ctx_s *p : c->parts) { gpu_backend_destroy(p->be); delete p; } // lanes[0] is parts[0]->be
+	} else gpu_backend_destroy(c->be);
 	if (c->d_resident) cudaFree(c->d_resident);
 	gpu_backend_trim_pool(c->device);
 	free_reg_vectors(c->res_regs);
@@ -210,10 +227,13 @@ extern "C" void wm_gpu_destroy(wm_gpu_ctx_s *c)
 // the pools stay resident (0.375 bytes per base) until the index is sketched, so that the -W list can be counted from them
 // first.  With H, the sequence table and the 4-bit host copy S are filled as well.
 struct ref_pools {
-	struct group { uint32_t *pk = 0, *nm = 0; int64_t *d_off = 0; std::vector<wm_sk_task> tasks; };
+	struct group {
+		uint32_t *pk = 0, *nm = 0; int64_t *d_off = 0; std::vector<wm_sk_task> tasks; int part = 0;
+		void release() { cudaFree(pk); cudaFree(nm); cudaFree(d_off); pk = nm = 0; d_off = 0; }
+	};
 	std::vector<group> g;
 	~ref_pools() { release(); }
-	void release() { for (auto &x : g) { cudaFree(x.pk); cudaFree(x.nm); cudaFree(x.d_off); } g.clear(); }
+	void release() { for (auto &x : g) x.release(); g.clear(); }
 	std::vector<wm_tf_group> tf() const
 	{
 		std::vector<wm_tf_group> v;
@@ -222,15 +242,39 @@ struct ref_pools {
 	}
 };
 
-static bool read_ref_pools(const char *ref_fn, wm_host_idx *H, ref_pools &P)
+// Where mm_idx_gen ends an index part (src/index.c:289-297 and :660-671, src/bseq.c:80-119): a part is read in mini-batches
+// of min(mini_batch_size, batch_size) bases, each mini-batch whole sequences until it holds at least that many bases, and
+// no further mini-batch is started once the part holds more than batch_size bases.
+struct PartCutter {
+	uint64_t batch, mb, part_sum = 0, mb_sum = 0;
+	bool open = false; // a mini-batch is being filled
+	int part = -1;
+	PartCutter(uint64_t batch_size, int mini_batch_size) : batch(batch_size), mb((uint64_t)mini_batch_size < batch_size ? (uint64_t)mini_batch_size : batch_size) {}
+	int next(uint64_t len) // the part of the next sequence
+	{
+		if (!open) {
+			if (part < 0 || part_sum > batch) ++part, part_sum = 0;
+			open = true, mb_sum = 0;
+		}
+		mb_sum += len;
+		if (mb_sum >= mb) part_sum += mb_sum, open = false;
+		return part;
+	}
+};
+
+// H (if not null) gets one sequence table per part: rid and offset restart at 0 in every part
+static bool read_ref_pools(const char *ref_fn, std::vector<wm_host_idx> *H, uint64_t batch_size, int mini_batch_size, ref_pools &P)
 {
 	SeqReader rd;
 	if (!rd.open(ref_fn)) { fprintf(stderr, "ERROR: failed to open file '%s'\n", ref_fn); return false; }
 	std::vector<wm_sk_task> tasks; std::string group; uint64_t sum_len = 0; uint32_t n_seq = 0;
+	PartCutter cut(batch_size, mini_batch_size);
+	int part = -1;
 	wm_dbuf d_ascii;
 	auto flush = [&]() {
 		if (tasks.empty()) return;
 		ref_pools::group G;
+		G.part = part;
 		const int64_t n = (int64_t)group.size();
 		char *da = (char*)d_ascii.need(group.size() + 16);
 		G.pk = wm_dev_alloc<uint32_t>(wm_pk_words(n)), G.nm = wm_dev_alloc<uint32_t>(wm_nm_words(n));
@@ -247,12 +291,19 @@ static bool read_ref_pools(const char *ref_fn, wm_host_idx *H, ref_pools &P)
 	};
 	wm_read r;
 	while (rd.next(r)) {
+		const int p = cut.next(r.seq.size());
+		if (p != part) {
+			flush();
+			part = p, sum_len = 0, n_seq = 0;
+			if (H) H->emplace_back();
+		}
 		const uint32_t rid = n_seq++;
 		if (H) {
-			H->name.push_back(r.name); H->len.push_back((uint32_t)r.seq.size()); H->offset.push_back(sum_len);
+			wm_host_idx *h = &H->back();
+			h->name.push_back(r.name); h->len.push_back((uint32_t)r.seq.size()); h->offset.push_back(sum_len);
 			const uint64_t need_words = (sum_len + r.seq.size() + 7) / 8;
-			if (H->S.size() < need_words) H->S.resize(need_words, 0);
-			pack_seq4(H->S.data(), sum_len, r.seq.data(), r.seq.size());
+			if (h->S.size() < need_words) h->S.resize(need_words, 0);
+			pack_seq4(h->S.data(), sum_len, r.seq.data(), r.seq.size());
 		}
 		sum_len += r.seq.size();
 		if (!r.seq.empty()) {
@@ -274,84 +325,153 @@ static bool distinct_ok(const char *who, double d)
 	return false;
 }
 
+static wm_gpu_ctx_s *new_ctx(int device)
+{
+	wm_gpu_ctx_s *c = new wm_gpu_ctx_s();
+	memset(&c->stats, 0, sizeof(c->stats));
+	c->device = device; c->t_index = c->t_map = 0;
+	return c;
+}
+
+// One index from the groups of part `part` of P (the groups are freed once sketched): the minimizers stay on the device,
+// where they are sorted and cut into the CSR (index_dev.cu).
+static wm_gpu_ctx_s *build_part(wm_host_idx &&H, ref_pools &P, int part, const wm_bloom_dev &bf, wm_bloom_s *bloom, int device)
+{
+	wm_gpu_ctx_s *c = new_ctx(device);
+	c->hidx = std::move(H);
+	const int k = c->hidx.k, w = c->hidx.w;
+	std::vector<std::pair<wm128_dev*, int64_t>> sk; int64_t n_mz_total = 0;
+	{
+		wm_sketch_ws ws;
+		for (auto &G : P.g) {
+			if (G.part != part) continue;
+			wm_pkseq pks; pks.pk = G.pk, pks.nm = G.nm;
+			int64_t n_mz = 0;
+			if (c->hidx.flag & WM_I_HPC) wm_sketch_run_hpc(&ws, bf, pks, G.tasks.data(), (int)G.tasks.size(), w, k, &n_mz, 0);
+			else wm_sketch_run(&ws, bf, pks, G.tasks.data(), (int)G.tasks.size(), w, k, &n_mz, 0);
+			WM_CUDA_CHECK(cudaDeviceSynchronize());
+			if (n_mz > 0) {
+				wm128_dev *d = wm_dev_alloc<wm128_dev>(n_mz);
+				WM_CUDA_CHECK(cudaMemcpy(d, ws.mz.p, sizeof(wm128_dev) * n_mz, cudaMemcpyDeviceToDevice));
+				sk.push_back(std::make_pair(d, n_mz)); n_mz_total += n_mz;
+			}
+			G.release();
+		}
+	}
+	set_name_order(&c->hidx);
+	// one array in position order, then sort + CSR on the device
+	wm128_dev *d_all = wm_dev_alloc<wm128_dev>(n_mz_total + 1);
+	{
+		int64_t o = 0;
+		for (auto &pp : sk) { WM_CUDA_CHECK(cudaMemcpy(d_all + o, pp.first, sizeof(wm128_dev) * pp.second, cudaMemcpyDeviceToDevice)); o += pp.second; cudaFree(pp.first); }
+	}
+	uint64_t *d_keys = 0, *d_poff = 0, *d_pos = 0; int64_t n_keys = 0;
+	wm_index_build_dev(d_all, n_mz_total, k, &d_keys, &d_poff, &d_pos, &n_keys, 0);
+	c->n_keys = n_keys, c->n_pos = n_mz_total;
+	c->be = gpu_backend_create_dev(&c->hidx, d_keys, n_keys, d_poff, d_pos, wm_bloom_bits(bloom), wm_bloom_table(bloom), device);
+	c->bloom_bits = wm_bloom_bits(bloom);
+	c->bloom.assign(wm_bloom_table(bloom), wm_bloom_table(bloom) + c->bloom_bits / 8);
+	return c;
+}
+
 // Index construction from a FASTA file (mm_idx_gen, src/index.c:378-449): same minimizers as the reference
 // because the reference sequences go through the same sketch kernel as the reads.  With WM_I_HPC the minimizers are
 // those of the homopolymer-compressed sequences (mm_sketch with is_hpc, src/index.c:347); S stays uncompressed.
 // The -W list comes from kmer_freq_fn, or, with distinct > 0, is counted on the device from the packed reference itself
-// (uncompressed also under WM_I_HPC: the list a user gets from meryl on ref.fa).
-static wm_gpu_ctx_s *index_build(const char *who, const char *ref_fn, const char *kmer_freq_fn, double distinct, int k, int w, int idx_flag, int device)
+// (uncompressed also under WM_I_HPC: the list a user gets from meryl on ref.fa).  The reference is cut into parts of about
+// batch_size bases as mm_idx_gen cuts it (PartCutter); UINT64_MAX gives one index whatever the size.  The FASTA is read,
+// the -W list counted and the filter built once for all parts.
+static wm_gpu_ctx_s *index_build(const char *who, const char *ref_fn, const char *kmer_freq_fn, double distinct, int k, int w, int idx_flag,
+                                 uint64_t batch_size, int mini_batch_size, int device)
 {
 	require_device(who);
 	if (!kw_ok(who, k, w) || !idx_flag_ok(who, idx_flag) || (distinct != 0.0 && !distinct_ok(who, distinct))) return 0;
 	WM_CUDA_CHECK(cudaSetDevice(device));
 	const double t0 = now_s();
-	wm_gpu_ctx_s *c = new wm_gpu_ctx_s();
-	memset(&c->stats, 0, sizeof(c->stats));
-	c->device = device; c->t_index = c->t_map = 0;
-	wm_host_idx &H = c->hidx;
-	H.k = k, H.w = w, H.flag = idx_flag;
+	std::vector<wm_host_idx> Hs;
 	ref_pools P;
-	if (!read_ref_pools(ref_fn, &H, P)) { delete c; return 0; }
+	if (!read_ref_pools(ref_fn, &Hs, batch_size, mini_batch_size, P)) return 0;
+	if (Hs.empty()) Hs.emplace_back(); // an empty reference: one empty index
+	for (auto &H : Hs) H.k = k, H.w = w, H.flag = idx_flag;
 	std::vector<uint64_t> kmers;
+	int64_t n_topfreq = 0; uint64_t topfreq_thr = 0; double t_topfreq = 0;
 	if (distinct != 0.0) {
 		const double tc = now_s();
 		wm_tf_list L;
 		wm_topfreq_dev(P.tf(), k, distinct, &L, 0);
 		kmers.swap(L.codes);
-		c->n_topfreq = (int64_t)kmers.size(), c->topfreq_thr = L.threshold, c->t_topfreq = now_s() - tc;
+		n_topfreq = (int64_t)kmers.size(), topfreq_thr = L.threshold, t_topfreq = now_s() - tc;
 	} else if (read_kmer_list(kmer_freq_fn, k, kmers) < 0) abort();
 	wm_bloom_s *bloom = wm_bloom_build(kmers.empty() ? 0 : kmers.data(), (int64_t)kmers.size());
 	uint8_t *d_table = wm_dev_alloc<uint8_t>(wm_bloom_bits(bloom) / 8 + 16);
 	WM_CUDA_CHECK(cudaMemcpy(d_table, wm_bloom_table(bloom), wm_bloom_bits(bloom) / 8, cudaMemcpyHostToDevice));
 	wm_bloom_dev bf; wm_bloom_dev_from_table(&bf, d_table, wm_bloom_bits(bloom));
-	// sketch every group; the minimizers stay on the device: they are sorted and cut into the CSR there (index_dev.cu)
-	std::vector<std::pair<wm128_dev*, int64_t>> parts; int64_t n_mz_total = 0;
-	wm_sketch_ws ws;
-	for (auto &G : P.g) {
-		wm_pkseq pks; pks.pk = G.pk, pks.nm = G.nm;
-		int64_t n_mz = 0;
-		if (idx_flag & WM_I_HPC) wm_sketch_run_hpc(&ws, bf, pks, G.tasks.data(), (int)G.tasks.size(), w, k, &n_mz, 0);
-		else wm_sketch_run(&ws, bf, pks, G.tasks.data(), (int)G.tasks.size(), w, k, &n_mz, 0);
-		WM_CUDA_CHECK(cudaDeviceSynchronize());
-		if (n_mz > 0) {
-			wm128_dev *part = wm_dev_alloc<wm128_dev>(n_mz);
-			WM_CUDA_CHECK(cudaMemcpy(part, ws.mz.p, sizeof(wm128_dev) * n_mz, cudaMemcpyDeviceToDevice));
-			parts.push_back(std::make_pair(part, n_mz)); n_mz_total += n_mz;
-		}
-	}
-	set_name_order(&H);
-	ws.release(); P.release(); cudaFree(d_table);
-	// one array in position order, then sort + CSR on the device
-	wm128_dev *d_all = wm_dev_alloc<wm128_dev>(n_mz_total + 1);
-	{
-		int64_t o = 0;
-		for (auto &pp : parts) { WM_CUDA_CHECK(cudaMemcpy(d_all + o, pp.first, sizeof(wm128_dev) * pp.second, cudaMemcpyDeviceToDevice)); o += pp.second; cudaFree(pp.first); }
-	}
-	uint64_t *d_keys = 0, *d_poff = 0, *d_pos = 0; int64_t n_keys = 0;
-	wm_index_build_dev(d_all, n_mz_total, k, &d_keys, &d_poff, &d_pos, &n_keys, 0);
-	c->n_keys = n_keys, c->n_pos = n_mz_total;
-	c->be = gpu_backend_create_dev(&H, d_keys, n_keys, d_poff, d_pos, wm_bloom_bits(bloom), wm_bloom_table(bloom), device);
-	c->bloom_bits = wm_bloom_bits(bloom);
-	c->bloom.assign(wm_bloom_table(bloom), wm_bloom_table(bloom) + c->bloom_bits / 8);
+	std::vector<wm_gpu_ctx_s*> parts;
+	for (size_t p = 0; p < Hs.size(); ++p) parts.push_back(build_part(std::move(Hs[p]), P, (int)p, bf, bloom, device));
+	P.release(); cudaFree(d_table);
 	wm_bloom_destroy(bloom);
+	wm_gpu_ctx_s *c = parts[0];
+	if (parts.size() > 1) { // the root: the sequence table of all parts, in part order (the merged index of mm_split_merge_prep)
+		c = new_ctx(device);
+		c->hidx.k = k, c->hidx.w = w, c->hidx.flag = idx_flag;
+		c->n_keys = c->n_pos = 0;
+		for (wm_gpu_ctx_s *p : parts) {
+			c->hidx.name.insert(c->hidx.name.end(), p->hidx.name.begin(), p->hidx.name.end());
+			c->hidx.len.insert(c->hidx.len.end(), p->hidx.len.begin(), p->hidx.len.end());
+			c->n_keys += p->n_keys, c->n_pos += p->n_pos;
+			p->root = c;
+		}
+		c->parts = parts;
+		c->be = parts[0]->be;
+	}
+	c->n_topfreq = n_topfreq, c->topfreq_thr = topfreq_thr, c->t_topfreq = t_topfreq;
 	c->t_index = now_s() - t0;
 	return c;
 }
 
 extern "C" wm_gpu_ctx_s *wm_index_build(const char *ref_fn, const char *kmer_freq_fn, int k, int w, int device)
 {
-	return index_build("wm_index_build", ref_fn, kmer_freq_fn, 0.0, k, w, 0, device);
+	return index_build("wm_index_build", ref_fn, kmer_freq_fn, 0.0, k, w, 0, UINT64_MAX, 0, device);
 }
 
 extern "C" wm_gpu_ctx_s *wm_index_build_opt(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, int device)
 {
-	return index_build("wm_index_build_opt", ref_fn, kmer_freq_fn, 0.0, io->k, io->w, io->flag, device);
+	return index_build("wm_index_build_opt", ref_fn, kmer_freq_fn, 0.0, io->k, io->w, io->flag, UINT64_MAX, 0, device);
 }
 
 extern "C" wm_gpu_ctx_s *wm_index_build_topfreq(const char *ref_fn, const wm_idxopt_t *io, double distinct, int device)
 {
 	if (!distinct_ok("wm_index_build_topfreq", distinct)) return 0;
-	return index_build("wm_index_build_topfreq", ref_fn, 0, distinct, io->k, io->w, io->flag, device);
+	return index_build("wm_index_build_topfreq", ref_fn, 0, distinct, io->k, io->w, io->flag, UINT64_MAX, 0, device);
+}
+
+extern "C" wm_gpu_ctx_s *wm_index_build_parts(const char *ref_fn, const char *kmer_freq_fn, const wm_idxopt_t *io, double distinct, int device)
+{
+	if (distinct != 0.0 && kmer_freq_fn) { fprintf(stderr, "[ERROR] wm_index_build_parts: give either a -W file or distinct, not both\n"); return 0; }
+	return index_build("wm_index_build_parts", ref_fn, kmer_freq_fn, distinct, io->k, io->w, io->flag, io->batch_size, io->mini_batch_size, device);
+}
+
+extern "C" int wm_part_plan(const char *ref_fn, uint64_t batch_size, int mini_batch_size, int32_t *n_seq, int cap)
+{
+	SeqReader rd;
+	if (!rd.open(ref_fn)) { fprintf(stderr, "ERROR: failed to open file '%s'\n", ref_fn); return -1; }
+	PartCutter cut(batch_size, mini_batch_size);
+	std::vector<int32_t> n;
+	wm_read r;
+	while (rd.next(r)) {
+		const int p = cut.next(r.seq.size());
+		if (p >= (int)n.size()) n.push_back(0);
+		++n[p];
+	}
+	for (int i = 0; i < (int)n.size() && i < cap; ++i) n_seq[i] = n[i];
+	return (int)n.size();
+}
+
+extern "C" int wm_idx_n_parts(const wm_gpu_ctx_s *c) { return is_multi(c) ? (int)c->parts.size() : 1; }
+extern "C" wm_gpu_ctx_s *wm_idx_part(wm_gpu_ctx_s *c, int i)
+{
+	if (is_multi(c)) return i >= 0 && (size_t)i < c->parts.size() ? c->parts[i] : 0;
+	return i == 0 ? c : 0;
 }
 
 // meryl count k=K + meryl print greater-than distinct=D on ref_fn: the list's length; up to cap (code, count) pairs into
@@ -363,7 +483,7 @@ extern "C" int64_t wm_topfreq(const char *ref_fn, int k, double distinct, uint64
 	if (!distinct_ok("wm_topfreq", distinct)) return -1;
 	WM_CUDA_CHECK(cudaSetDevice(device));
 	ref_pools P;
-	if (!read_ref_pools(ref_fn, 0, P)) return -1;
+	if (!read_ref_pools(ref_fn, 0, UINT64_MAX, 0, P)) return -1;
 	wm_tf_list L;
 	wm_topfreq_dev(P.tf(), k, distinct, &L, 0);
 	const int64_t n = (int64_t)L.codes.size(), m = std::min<int64_t>(n, cap > 0 ? cap : 0);
@@ -374,6 +494,55 @@ extern "C" int64_t wm_topfreq(const char *ref_fn, int k, double distinct, uint64
 
 extern "C" int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo) { return set_opt(preset, io, mo); }
 extern "C" int wm_check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo) { return check_opt(io, mo); }
+// mm_idx_cal_max_occ (src/index.c:173-194) of one index: INT32_MAX for f <= 0, else the ((1 - f) * n)-th smallest occurrence
+// count over the n keys, plus one, selected on the device (occ_select.cu) and remembered per f.  -1, with a message, where
+// the reference would read past its array (the rank reaches n: f too small for the number of keys, or no key at all) and
+// on a multi-part context, whose parts each have their own value.
+extern "C" int32_t wm_idx_cal_max_occ(const wm_gpu_ctx_s *c_, float f)
+{
+	wm_gpu_ctx_s *c = const_cast<wm_gpu_ctx_s*>(c_);
+	if (f <= 0.) return INT32_MAX;
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_idx_cal_max_occ: a multi-part index has one value per part (wm_idx_part)\n"); return -1; }
+	std::lock_guard<std::mutex> lk(c->occ_mu);
+	for (auto &e : c->occ_cache) if (e.first == f) return e.second;
+	const uint64_t n = (uint64_t)c->n_keys, rank = (uint32_t)((1. - f) * n);
+	if (rank >= n) {
+		fprintf(stderr, "[ERROR] wm_idx_cal_max_occ: f = %g selects rank %llu of %llu occurrence counts; the reference reads past its array here\n",
+		        (double)f, (unsigned long long)rank, (unsigned long long)n);
+		return -1;
+	}
+	WM_CUDA_CHECK(cudaSetDevice(c->device));
+	const uint64_t *dk, *dpo, *dp;
+	gpu_backend_index_arrays(c->be, &dk, &dpo, &dp);
+	const int32_t v = (int32_t)(wm_occ_select_dev(dpo, (int64_t)n, rank, 0) + 1);
+	c->occ_cache.push_back(std::make_pair(f, v));
+	return v;
+}
+
+// mm_mapopt_update (src/options.c:71-81) against one index; 0, or -1 when wm_idx_cal_max_occ refuses
+extern "C" int wm_mapopt_update(wm_mapopt_t *opt, const wm_gpu_ctx_s *c)
+{
+	if ((opt->flag & WM_F_SPLICE_FOR) || (opt->flag & WM_F_SPLICE_REV)) opt->flag |= WM_F_SPLICE;
+	if (opt->mid_occ_frac >= 0 && opt->mid_occ_frac < 1) {
+		const int32_t m = wm_idx_cal_max_occ(c, opt->mid_occ_frac);
+		if (m < 0) return -1;
+		opt->mid_occ = m;
+	}
+	if (opt->mid_occ < opt->min_mid_occ) opt->mid_occ = opt->min_mid_occ;
+	return 0;
+}
+
+// The options one index maps with: under -f, mid_occ of that index (what mm_mapopt_update sets per part, src/main.c:403);
+// without -f, opt unchanged.  false when the selection is refused.
+static bool part_opt(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, wm_mapopt_t *o)
+{
+	*o = *opt;
+	if (!(opt->mid_occ_frac >= 0 && opt->mid_occ_frac < 1)) return true;
+	if (wm_mapopt_update(o, c) < 0) return false;
+	o->mid_occ_frac = -1.0f; // resolved
+	return true;
+}
+
 extern "C" int wm_sizeof_mapopt(void) { return (int)sizeof(wm_mapopt_t); }
 extern "C" int wm_sizeof_reg1(void) { return (int)sizeof(wm_reg1_t); }
 extern "C" int wm_abi_layout(int64_t *out, int cap)
@@ -404,6 +573,45 @@ extern "C" int wm_abi_layout(int64_t *out, int cap)
 	return n;
 }
 
+// The parts of a context in order: its own index for a single one
+static std::vector<wm_gpu_ctx_s*> parts_of(wm_gpu_ctx_s *c) { return is_multi(c) ? c->parts : std::vector<wm_gpu_ctx_s*>(1, c); }
+
+// --split-prefix: every read mapped against every part, then merge_hits (src/map.c:1050-1105) in memory: the regs of the
+// parts concatenated in part order, rid shifted by the sequences of the earlier parts, then mm_hit_sort, mm_set_parent,
+// mm_select_sub and mm_set_sam_pri (not under MM_F_ALL_CHAINS) and mm_set_mapq with the largest rep_len of the parts.
+static bool map_merged(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads, std::vector<std::vector<wm_reg1_t>> &regs, int n_threads)
+{
+	const std::vector<wm_gpu_ctx_s*> parts = parts_of(c);
+	const int n = (int)reads.size();
+	regs.assign(n, std::vector<wm_reg1_t>());
+	std::vector<int> rep_len(n, 0);
+	int32_t rid_shift = 0;
+	for (wm_gpu_ctx_s *p : parts) {
+		wm_mapopt_t o;
+		if (!part_opt(p, opt, &o)) return false;
+		std::vector<std::vector<wm_reg1_t>> r; std::vector<int> rl, fg;
+		map_lanes(p, &o, reads, r, rl, fg, n_threads, false);
+		for (int i = 0; i < n; ++i) {
+			for (auto &x : r[i]) { x.rid += rid_shift; regs[i].push_back(x); }
+			rep_len[i] = std::max(rep_len[i], rl[i]);
+		}
+		rid_shift += (int32_t)p->hidx.name.size();
+	}
+	const int k = c->hidx.k;
+	#pragma omp parallel for schedule(dynamic, 16) num_threads(n_threads > 0 ? n_threads : 1)
+	for (int i = 0; i < n; ++i) {
+		std::vector<wm_reg1_t> &v = regs[i];
+		hit_sort(v, opt->alt_drop);
+		set_parent(opt->mask_level, opt->mask_len, (int)v.size(), v.data(), opt->a * 2 + opt->b, (int)(opt->flag & WM_F_HARD_MLEVEL), opt->alt_drop);
+		if (!(opt->flag & WM_F_ALL_CHAINS)) {
+			select_sub(opt->pri_ratio, k * 2, opt->best_n, v);
+			set_sam_pri((int)v.size(), v.data());
+		}
+		set_mapq(v, opt->min_chain_score, opt->a, rep_len[i], 0);
+	}
+	return true;
+}
+
 // The GPU replacement of kt_for(n_threads, worker_for, ...) (src/map.c:1164): fills n_reg/reg/rep_len/frag_gap of
 // every sequence exactly as worker_for does (:1025-1034).  reg[i] and each reg[i][j].p are malloc()ed; the caller
 // frees them (src/minimap.h:355-356).
@@ -421,7 +629,18 @@ extern "C" int wm_gpu_map_batch(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, int n_s
 		reads[i] = &store[i];
 	}
 	std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-	map_lanes(c, opt, reads, regs, rl, fg, n_threads, false);
+	if (is_multi(c)) {
+		if (!opt->split_prefix) {
+			fprintf(stderr, "[ERROR] wm_gpu_map_batch: a multi-part index maps part by part (wm_idx_part) unless split_prefix asks for merged hits\n");
+			return -1;
+		}
+		if (!map_merged(c, opt, reads, regs, n_threads)) return -1;
+		rl.assign(n_seq, 0), fg.assign(n_seq, 0);
+	} else {
+		wm_mapopt_t o;
+		if (!part_opt(c, opt, &o)) return -1;
+		map_lanes(c, &o, reads, regs, rl, fg, n_threads, false);
+	}
 	for (int i = 0; i < n_seq; ++i) {
 		n_reg[i] = (int32_t)regs[i].size();
 		reg[i] = 0;
@@ -455,21 +674,18 @@ extern "C" wm_reg1_t *wm_map(wm_gpu_ctx_s *c, int l_seq, const char *seq, int *n
 // length descending inside a batch (src/map.c:1124-1143) and printed in that order (:1173-1208).  With world > 1
 // this process maps and prints only the reads whose position in the sorted batch is rank mod world; every output
 // line is preceded by "<batch>\t<position>\t" when tag_order != 0 so that the shards can be merged back.
-extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, int n_threads, int rank, int world,
-                           int tag_order, int64_t max_batch_bases)
+// One pass over the read file: c is one index (mapped and written as mm_map_file does), or, with `merged`, the context whose
+// parts are all mapped and merged per read (map_merged), written with the sequence table of all parts.
+static int map_file_pass(wm_gpu_ctx_s *c, const wm_mapopt_t *opt_in, const char *reads_fn, FILE *out, int n_threads, int rank, int world,
+                         int tag_order, int64_t max_batch_bases, bool merged)
 {
-	require_device("wm_map_file");
 	SeqReader rd;
 	if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
-	FILE *out = out_fn && strcmp(out_fn, "-") ? fopen(out_fn, "wb") : stdout;
-	if (!out) return -1;
-	const double t0 = now_s();
+	wm_mapopt_t opt_part;
+	if (!merged && !part_opt(c, opt_in, &opt_part)) return -1;
+	const wm_mapopt_t *opt = merged ? opt_in : &opt_part;
 	const int64_t chunk = opt->mini_batch_size;
-	if ((opt->flag & WM_F_OUT_SAM) && rank == 0 && !tag_order) { // mm_write_sam_hdr (src/main.c:391-393)
-		std::string hdr;
-		write_sam_hdr(hdr, &c->hidx, "2.03", c->sam_cl.c_str());
-		fwrite(hdr.data(), 1, hdr.size(), out);
-	}
+	bool failed = false;
 	// The three steps of the reference's pipeline (src/map.c:1107-1224: read, map, write) run on three threads with
 	// one mini-batch of slack between them: the next batch is parsed and the previous one formatted while the GPU maps.
 	struct FileBatch {
@@ -555,7 +771,11 @@ extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *
 			while (s1 < b->mine.size() && (s1 == s0 || nb + (int64_t)b->mine[s1]->seq.size() <= max_batch_bases)) nb += (int64_t)b->mine[s1]->seq.size(), ++s1;
 			std::vector<const wm_read*> sub(b->mine.begin() + s0, b->mine.begin() + s1);
 			std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-			map_lanes(c, opt, sub, regs, rl, fg, n_threads, false);
+			if (merged) { // the merge pass leaves rep_len 0 in what it prints (src/map.c:1050-1105 does not set it)
+				if (!failed && !map_merged(c, opt, sub, regs, n_threads)) failed = true;
+				if (failed) regs.assign(sub.size(), std::vector<wm_reg1_t>());
+				rl.assign(sub.size(), 0);
+			} else map_lanes(c, opt, sub, regs, rl, fg, n_threads, false);
 			for (size_t i = 0; i < sub.size(); ++i) { b->regs[s0 + i].swap(regs[i]); b->rl[s0 + i] = rl[i]; }
 			s0 = s1;
 		}
@@ -563,9 +783,44 @@ extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *
 	}
 	q_out.close();
 	reader.join(); writer.join();
+	return failed ? -1 : 0;
+}
+
+// Without split_prefix a multi-part index is mapped part by part and written part-major, as the reference's loop over the
+// parts does (src/main.c:384-424); the SAM header then has no @SQ line (mm_write_sam_hdr(0, ...), :391-398).  With
+// split_prefix the parts' hits are merged per read in one pass (mm_split_merge, src/map.c:1278-1321), also for a single
+// index: its @SQ lines then come twice, the normal header's and the merge's, as the reference prints them.  The reference
+// goes through temporary files <prefix>.NNNN.tmp; here the merge runs in memory and no file is written.
+extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, int n_threads, int rank, int world,
+                           int tag_order, int64_t max_batch_bases)
+{
+	require_device("wm_map_file");
+	const bool merged = opt->split_prefix != 0;
+	if (is_multi(c) && !merged && world > 1) {
+		fprintf(stderr, "[ERROR] wm_map_file: a multi-part index without split_prefix is written part-major, which does not shard over ranks\n");
+		return -1;
+	}
+	{ // the read file is checked before the output is created
+		SeqReader rd;
+		if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
+	}
+	FILE *out = out_fn && strcmp(out_fn, "-") ? fopen(out_fn, "wb") : stdout;
+	if (!out) return -1;
+	const double t0 = now_s();
+	if ((opt->flag & WM_F_OUT_SAM) && rank == 0 && !tag_order) { // mm_write_sam_hdr (src/main.c:391-398); the merge's @SQ lines follow (src/map.c:1304-1306)
+		std::string h;
+		wm_host_idx none;
+		write_sam_hdr(h, is_multi(c) ? &none : &c->hidx, "2.03", c->sam_cl.c_str());
+		if (merged)
+			for (size_t i = 0; i < c->hidx.name.size(); ++i) { h += "@SQ\tSN:"; h += c->hidx.name[i]; h += "\tLN:"; h += std::to_string(c->hidx.len[i]); h += '\n'; }
+		fwrite(h.data(), 1, h.size(), out);
+	}
+	int rc = 0;
+	if (merged) rc = map_file_pass(c, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases, true);
+	else for (wm_gpu_ctx_s *p : parts_of(c)) if (rc == 0) rc = map_file_pass(p, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases, false);
 	if (out != stdout) fclose(out); else fflush(out);
 	c->t_map += now_s() - t0;
-	return 0;
+	return rc;
 }
 
 extern "C" void wm_set_sam_cl(wm_gpu_ctx_s *c, const char *cl) { c->sam_cl = cl ? cl : ""; }
@@ -574,6 +829,7 @@ extern "C" void wm_set_sam_cl(wm_gpu_ctx_s *c, const char *cl) { c->sam_cl = cl 
 // small, *max_len is its capacity; the string is NUL terminated; returns its length
 static int gen_cs_or_md_c(const wm_gpu_ctx_s *c, char **buf, int *max_len, const wm_reg1_t *r, const char *seq, int is_MD, int no_iden)
 {
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_gen_cs / wm_gen_MD: the reference sequence is held by the parts of a multi-part index (wm_idx_part)\n"); return -1; }
 	std::string s;
 	gen_cs_or_MD(s, &c->hidx, r, seq, is_MD, no_iden);
 	if ((int)s.size() + 1 > *max_len) {
@@ -587,7 +843,11 @@ static int gen_cs_or_md_c(const wm_gpu_ctx_s *c, char **buf, int *max_len, const
 	return (int)s.size();
 }
 // mm_idx_getseq / mm_idx_name2id (src/index.c:161-171, :131-140) and the sequence table of the index (mm_idx_seq_t)
-extern "C" int wm_idx_getseq(const wm_gpu_ctx_s *c, uint32_t rid, uint32_t st, uint32_t en, uint8_t *seq) { return c->hidx.getseq(rid, st, en, seq); }
+extern "C" int wm_idx_getseq(const wm_gpu_ctx_s *c, uint32_t rid, uint32_t st, uint32_t en, uint8_t *seq)
+{
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_idx_getseq: the reference sequence is held by the parts of a multi-part index (wm_idx_part)\n"); return -1; }
+	return c->hidx.getseq(rid, st, en, seq);
+}
 extern "C" int wm_idx_name2id(const wm_gpu_ctx_s *c, const char *name)
 {
 	for (size_t i = 0; i < c->hidx.name.size(); ++i) if (c->hidx.name[i] == name) return (int)i;
@@ -650,6 +910,7 @@ extern "C" void wm_free_regs(int n, const int32_t *n_reg, wm_reg1_t **reg)
 // bench: put a batch of reads into HBM (ASCII -> codes, both strands) outside the timed region ...
 extern "C" int wm_bench_upload(wm_gpu_ctx_s *c, int n_seq, const char *const *names, const char *const *seqs, const int32_t *lens)
 {
+	if (is_multi(c) || c->root) { fprintf(stderr, "[ERROR] wm_bench_upload: resident reads are for a single index\n"); return -1; }
 	c->resident.assign(n_seq, wm_read());
 	int64_t tot = 0;
 	for (int i = 0; i < n_seq; ++i) {
@@ -780,6 +1041,7 @@ static void fetch_index_arrays(wm_gpu_ctx_s *c)
 extern "C" int64_t wm_idx_blob_size(const wm_gpu_ctx_s *c_)
 {
 	wm_gpu_ctx_s *c = const_cast<wm_gpu_ctx_s*>(c_);
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_idx_blob_size: the fan-out of a multi-part index is not supported\n"); return -1; }
 	fetch_index_arrays(c);
 	const wm_host_idx &H = c->hidx;
 	size_t names = 0;
@@ -791,6 +1053,7 @@ extern "C" int64_t wm_idx_blob_size(const wm_gpu_ctx_s *c_)
 extern "C" int wm_idx_blob_write(const wm_gpu_ctx_s *c_, uint8_t *buf)
 {
 	wm_gpu_ctx_s *c = const_cast<wm_gpu_ctx_s*>(c_);
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_idx_blob_write: the fan-out of a multi-part index is not supported\n"); return -1; }
 	fetch_index_arrays(c);
 	const wm_host_idx &H = c->hidx;
 	size_t names = 0;

@@ -270,6 +270,11 @@ void wm_chain_run(wm_chain_ws *ws, wm128_dev *d_a, const int64_t *d_off, const i
 	wm128_dev *w = (wm128_dev*)ws->w.need(sizeof(wm128_dev) * (n_a + 1)), *b = (wm128_dev*)ws->b.need(sizeof(wm128_dev) * (n_a + 1));
 	int32_t *n_u = (int32_t*)ws->n_u.need(sizeof(int32_t) * (n_tasks + 1));
 	int64_t *n_b = (int64_t*)ws->n_b.need(sizeof(int64_t) * (n_tasks + 1));
+	if (n_a == 0) { // no task has an anchor (a wave of reads without a seed hit in this index): no chain, and no launch of size 0
+		WM_CUDA_CHECK(cudaMemsetAsync(n_u, 0, sizeof(int32_t) * n_tasks, st));
+		WM_CUDA_CHECK(cudaMemsetAsync(n_b, 0, sizeof(int64_t) * n_tasks, st));
+		return;
+	}
 	int *counter = (int*)ws->counter.need(8 * sizeof(int));
 	WM_CUDA_CHECK(cudaMemsetAsync(counter, 0, 8 * sizeof(int), st));
 	// largest tasks first

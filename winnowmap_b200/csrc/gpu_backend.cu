@@ -106,6 +106,9 @@ struct GpuBackendImpl {
 	wm_hbuf<uint32_t> h_cig; wm_hbuf<wm_extz_dev> h_ez; wm_hbuf<int32_t> h_zd; wm_dbuf zd;
 	size_t bt_budget;
 	bool owns_index = false; // the lane that uploaded the index frees it; clones only borrow the pointers
+	// the index this backend was created with (ix / bf / hidx above are the one it maps against, which gpu_backend_bind
+	// may point at another index of the same context: one part of a multi-part index)
+	wm_idx_dev own_ix; wm_bloom_dev own_bf; const wm_host_idx *own_hidx;
 };
 
 class GpuBackend : public Backend {
@@ -119,9 +122,10 @@ public:
 		if (g.dpws.fill_st) cudaStreamSynchronize(g.dpws.fill_st);
 		if (g.h_stage) cudaFreeHost(g.h_stage);
 		if (g.owns_index) {
-			cudaFree((void*)g.ix.keys); cudaFree((void*)g.ix.pos_off); cudaFree((void*)g.ix.pos); cudaFree((void*)g.ix.S);
-			cudaFree((void*)g.ix.ht_key); cudaFree((void*)g.ix.ht_val); cudaFree((void*)g.bf.table);
-			cudaFree((void*)g.ix.seq_len); cudaFree((void*)g.ix.name_rank);
+			const wm_idx_dev &x = g.own_ix;
+			cudaFree((void*)x.keys); cudaFree((void*)x.pos_off); cudaFree((void*)x.pos); cudaFree((void*)x.S);
+			cudaFree((void*)x.ht_key); cudaFree((void*)x.ht_val); cudaFree((void*)g.own_bf.table);
+			cudaFree((void*)x.seq_len); cudaFree((void*)x.name_rank);
 		}
 		if (g.st) cudaStreamDestroy(g.st);
 		// this thread's workspace allocations must not go on to the stream just destroyed (wm_dbuf_use_stream)
@@ -681,6 +685,7 @@ Backend *gpu_backend_create_dev(const wm_host_idx *hidx, uint64_t *d_keys, int64
 	wm_idx_dev_build_ht(&g.ix, g.st);
 	wm_bloom_dev_from_table(&g.bf, d_bt, bloom_bits);
 	g.owns_index = true;
+	g.own_ix = g.ix, g.own_bf = g.bf, g.own_hidx = hidx;
 	wm_stream_sync(g.st);
 	size_t free_b = 0, total_b = 0;
 	WM_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
@@ -720,7 +725,16 @@ Backend *gpu_backend_create(const wm_host_idx *hidx, const uint64_t *keys, int64
 void gpu_backend_index_arrays(Backend *be_, const uint64_t **d_keys, const uint64_t **d_poff, const uint64_t **d_pos)
 {
 	GpuBackend *be = static_cast<GpuBackend*>(be_);
-	*d_keys = be->g.ix.keys, *d_poff = be->g.ix.pos_off, *d_pos = be->g.ix.pos;
+	*d_keys = be->g.own_ix.keys, *d_poff = be->g.own_ix.pos_off, *d_pos = be->g.own_ix.pos;
+}
+
+// Point a lane at the index `src` was created with (one part of a multi-part index): the lane keeps its stream and
+// workspaces, which depend on no index.  The caller makes sure no batch of the lane is in flight.
+void gpu_backend_bind(Backend *lane_, const Backend *src_)
+{
+	GpuBackendImpl &g = static_cast<GpuBackend*>(lane_)->g;
+	const GpuBackendImpl &s = static_cast<const GpuBackend*>(src_)->g;
+	g.ix = s.own_ix, g.bf = s.own_bf, g.hidx = s.own_hidx;
 }
 
 // A second orchestration lane on the same device: shares the resident index, owns its stream and workspaces.
@@ -732,6 +746,7 @@ Backend *gpu_backend_clone(Backend *base_, int n_lanes)
 	GpuBackendImpl &g = be->g;
 	g.device = base->g.device; g.hidx = base->g.hidx; g.n_bases = 0;
 	g.ix = base->g.ix; g.bf = base->g.bf;
+	g.own_ix = base->g.own_ix, g.own_bf = base->g.own_bf, g.own_hidx = base->g.own_hidx;
 	g.st = wm_stream_create_high_priority(); // the DP fill kernels go to a lowest-priority side stream (wm_extd2_launch)
 	g.bt_budget = base->g.bt_budget / (size_t)(n_lanes > 0 ? n_lanes : 1);
 	return be;

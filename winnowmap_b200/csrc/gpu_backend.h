@@ -9,7 +9,10 @@ Backend *gpu_backend_create(const wm_host_idx *hidx, const uint64_t *keys, int64
 // the same with the index arrays already on the device (ownership passes to the backend)
 Backend *gpu_backend_create_dev(const wm_host_idx *hidx, uint64_t *d_keys, int64_t n_keys, uint64_t *d_poff, uint64_t *d_pos,
                                 uint64_t bloom_bits, const uint8_t *bloom_table, int device);
+// the index arrays the backend was created with (not those of the index gpu_backend_bind points it at)
 void gpu_backend_index_arrays(Backend *be, const uint64_t **d_keys, const uint64_t **d_poff, const uint64_t **d_pos);
+// map with the index another backend was created with (a part of the same multi-part index); streams and workspaces stay
+void gpu_backend_bind(Backend *lane, const Backend *src);
 void gpu_backend_destroy(Backend *be);
 }
 

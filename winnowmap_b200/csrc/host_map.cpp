@@ -148,8 +148,8 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		fprintf(stderr, "[ERROR] winnowmap-b200: max_qlen is not implemented\n");
 		exit(1);
 	}
-	if (opt->mid_occ_frac >= 0.0f && opt->mid_occ_frac < 1.0f) { // -f: mm_mapopt_update would derive mid_occ from the index (src/options.c:75-76)
-		fprintf(stderr, "[ERROR] winnowmap-b200: mid_occ_frac (-f) is not implemented: set mid_occ itself\n");
+	if (opt->mid_occ_frac >= 0.0f && opt->mid_occ_frac < 1.0f) { // -f: the C ABI resolves it per index (wm_mapopt_update) before mapping
+		fprintf(stderr, "[ERROR] winnowmap-b200: mid_occ_frac (-f) reached the batch unresolved: set mid_occ from the index first (wm_mapopt_update)\n");
 		exit(1);
 	}
 	const double t_batch0 = Timers::now();

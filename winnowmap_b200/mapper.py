@@ -51,6 +51,15 @@ def _setup(L):
     L.wm_topfreq.argtypes = [C.c_char_p, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64), C.c_int]
     L.wm_topfreq_threshold.restype = C.c_uint64
     L.wm_topfreq_threshold.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_double]
+    L.wm_index_build_parts.restype = C.c_void_p
+    L.wm_index_build_parts.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(IdxOpt), C.c_double, C.c_int]
+    L.wm_idx_n_parts.argtypes = [C.c_void_p]
+    L.wm_idx_part.restype = C.c_void_p
+    L.wm_idx_part.argtypes = [C.c_void_p, C.c_int]
+    L.wm_part_plan.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.c_void_p, C.c_int]
+    L.wm_idx_cal_max_occ.restype = C.c_int32
+    L.wm_idx_cal_max_occ.argtypes = [C.c_void_p, C.c_float]
+    L.wm_mapopt_update.argtypes = [C.POINTER(MapOpt), C.c_void_p]
     L.wm_idx_flag.argtypes = [C.c_void_p]
     L.wm_gpu_destroy.argtypes = [C.c_void_p]
     L.wm_idx_blob_size.restype = C.c_int64
@@ -105,22 +114,41 @@ class Mapper:
     --for-only / --rev-only): Mapper(reads, preset="map-ont", all_vs_all=True).map_file(reads, out) computes overlaps.
     distinct=D takes the -W list from the reference itself instead of the file kmer_freq: the k-mers that
     `meryl count k=K` + `meryl print greater-than distinct=D` list (top_kmers), counted on the GPU; 0.9998 is the
-    reference README's recipe."""
+    reference README's recipe.
+    part_bases is -I: the reference is cut into index parts of about that many bases (wm_index_build_parts), which stay on the
+    GPU together; the output is then part-major, or, with split=True (--split-prefix), the parts' hits are merged per read
+    in memory (no temporary file is written).  mid_occ_frac is -f: each index part gets its own mid_occ, selected on the
+    GPU from its occurrence counts."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
-                 no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None):
+                 no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
             raise ValueError(f"distinct must be in (0, 1], not {distinct!r}")
+        if part_bases is not None and (blob is not None or int(part_bases) <= 0):
+            raise ValueError("part_bases must be a positive number of bases and cannot be combined with blob=")
+        if mid_occ_frac is not None and not 0.0 <= mid_occ_frac < 1.0:
+            raise ValueError(f"mid_occ_frac must be in [0, 1), not {mid_occ_frac!r}")
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand)
         if hpc:
             self.io.flag |= I_HPC
+        if mid_occ_frac is not None:
+            self.mo.mid_occ_frac = mid_occ_frac
+        if split:
+            self.mo.split_prefix = b"split"  # any prefix: the merge runs in memory and writes no file
+            rc = self.L.wm_check_opt(C.byref(self.io), C.byref(self.mo))
+            if rc < 0:
+                raise ValueError(f"mm_check_opt-style validation failed: {rc}")
         self.n_threads = n_threads or max(1, min(64, (os.cpu_count() or 2) // 2))
         if blob is not None:  # index received from another rank (numpy uint8 array)
             self._blob_keep = blob
             self.ctx = self.L.wm_idx_blob_load(blob.ctypes.data, blob.nbytes, device)
+        elif part_bases is not None:
+            self.io.batch_size = int(part_bases)
+            self.ctx = self.L.wm_index_build_parts(ref.encode(), kmer_freq.encode() if kmer_freq else None, C.byref(self.io),
+                                                   float(distinct or 0.0), device)
         elif distinct is not None:
             self.ctx = self.L.wm_index_build_topfreq(ref.encode(), C.byref(self.io), float(distinct), device)
         else:
@@ -133,9 +161,16 @@ class Mapper:
         """True when the index holds homopolymer-compressed minimizers (MM_I_HPC)."""
         return bool(self.L.wm_idx_flag(self.ctx) & I_HPC)
 
+    @property
+    def n_parts(self):
+        """The number of index parts (1 unless part_bases cut the reference)."""
+        return self.L.wm_idx_n_parts(self.ctx)
+
     def index_blob(self):
         """The flattened index as one numpy uint8 array (for the one-time NCCL fan-out)."""
         import numpy as np
+        if self.n_parts > 1:
+            raise RuntimeError("the blob fan-out of a multi-part index is not supported")
         n = self.L.wm_idx_blob_size(self.ctx)
         buf = np.empty(n, dtype=np.uint8)
         self.L.wm_idx_blob_write(self.ctx, buf.ctypes.data)
@@ -164,6 +199,21 @@ class Mapper:
             self.close()
         except Exception:
             pass
+
+
+def part_plan(ref, part_bases, mini_batch_size=50_000_000):
+    """The number of sequences in each index part that part_bases (-I) gives, on the host: the plan wm_index_build_parts
+    follows and the reference's index reader cuts (no GPU needed)."""
+    L = _setup(lib())
+    cap = 1
+    while True:
+        buf = (C.c_int32 * cap)()
+        n = L.wm_part_plan(ref.encode(), int(part_bases), int(mini_batch_size), buf, cap)
+        if n < 0:
+            raise RuntimeError(f"cannot read {ref}")
+        if n <= cap:
+            return list(buf[:n])
+        cap = n
 
 
 def top_kmers(ref, k, distinct=0.9998, device=0):
