@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY (lives under tests/, never shipped): a Backend whose three device operations are
 // served by the CPU oracle (oracle/wm_oracle.c).  Linked with the product's *host* sources it lets the CPU-only
-// test-suite drive the whole orchestration (host_map / host_align / host_glue / host_format) end to end and
-// compare the PAF with the reference goldens -- the product library itself never contains or loads this.
+// test-suite drive the whole orchestration (host_driver / host_map / host_align / host_glue / host_format) end to end
+// and compare the PAF with the reference goldens -- the product library itself never contains or loads this.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -9,6 +9,8 @@
 #include <string>
 #include <vector>
 #include "../../winnowmap_b200/csrc/host_backend.h"
+#include "../../winnowmap_b200/csrc/host_driver.h"
+#include "../../winnowmap_b200/csrc/host_index.h"
 #include "../../winnowmap_b200/csrc/host_io.h"
 
 extern "C" {
@@ -189,71 +191,116 @@ struct OracleIndex {
 	~OracleIndex() { if (bloom) wmo_bloom_free(bloom); }
 };
 
-static int load_oracle_index(const char *ref_fn, const char *kmer_fn, int k, int w, OracleIndex &X)
+// the -W list of kmer_fn and its down-weight filter
+static int load_kmer_filter(const char *kmer_fn, int k, OracleIndex &X)
 {
-	wm_host_idx &H = X.H;
-	H.k = k, H.w = w;
 	if (read_kmer_list(kmer_fn, k, X.kmers) < 0) return -3;
 	X.bloom = wmo_bloom_init(X.kmers.size());
 	for (uint64_t km : X.kmers) wmo_bloom_insert(X.bloom, km);
-	SeqReader rd;
-	if (!rd.open(ref_fn)) return -4;
-	wm_read r; uint64_t sum_len = 0;
-	while (rd.next(r)) {
-		const uint32_t rid = (uint32_t)H.name.size();
-		H.name.push_back(r.name); H.len.push_back((uint32_t)r.seq.size()); H.offset.push_back(sum_len);
-		H.S.resize((sum_len + r.seq.size() + 7) / 8, 0);
-		for (size_t j = 0; j < r.seq.size(); ++j) { uint64_t o = sum_len + j; uint8_t c = code_of(r.seq[j]); if (r.seq[j] == 'U' || r.seq[j] == 'u') c = 4; H.S[o >> 3] |= (uint32_t)c << ((o & 7) << 2); }
-		sum_len += r.seq.size();
-		if (r.seq.empty()) continue;
-		std::vector<uint64_t> tmp((size_t)2 * (r.seq.size() / 2 + 64));
-		long n = wmo_sketch(r.seq.data(), (int)r.seq.size(), w, k, rid, X.bloom, tmp.data(), (long)tmp.size() / 2);
-		X.mz.insert(X.mz.end(), tmp.begin(), tmp.begin() + 2 * n);
-	}
 	return 0;
 }
 
-// Maps every read of `reads_fn` through `be` (one batch, longest reads first) and writes PAF or SAM to `out_fn`.
-static int map_reads_to(Backend *be, const wm_host_idx &H, const wm_mapopt_t &mo, const char *reads_fn, const char *out_fn, int n_threads, int sam)
+// The sequences of index part `part` of ref_fn, cut as mm_idx_gen cuts it (PartCutter; the defaults give one part), sketched
+// with the filter `bloom`: the number of parts of the file, or < 0 when it cannot be read
+static int load_oracle_seqs(const char *ref_fn, int k, int w, const void *bloom, OracleIndex &X, uint64_t part_bases = UINT64_MAX,
+                            int mini_batch_size = 0, int part = 0)
 {
+	wm_host_idx &H = X.H;
+	H.k = k, H.w = w;
 	SeqReader rd;
-	if (!rd.open(reads_fn)) return -5;
-	std::vector<wm_read> batch; wm_read r;
-	while (rd.next(r)) batch.push_back(r);
-	std::vector<std::pair<int, int>> ord;
-	for (size_t i = 0; i < batch.size(); ++i) ord.emplace_back((int)batch[i].seq.size(), (int)i);
-	std::sort(ord.begin(), ord.end(), std::greater<std::pair<int, int>>());
-	std::vector<const wm_read*> reads;
-	for (auto &o : ord) reads.push_back(&batch[o.second]);
-	std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-	map_batch(be, &H, &mo, reads, regs, rl, fg, n_threads, 0);
-	FILE *out = fopen(out_fn, "wb");
-	std::string line;
+	if (!rd.open(ref_fn)) return -4;
+	PartCutter cut(part_bases, mini_batch_size);
+	int n_parts = 0;
+	wm_read r; uint64_t sum_len = 0;
+	while (rd.next(r)) {
+		n_parts = cut.next(r.seq.size()) + 1;
+		if (n_parts - 1 != part) continue;
+		const uint32_t rid = (uint32_t)H.name.size();
+		H.name.push_back(r.name); H.len.push_back((uint32_t)r.seq.size()); H.offset.push_back(sum_len);
+		H.S.resize((sum_len + r.seq.size() + 7) / 8, 0);
+		pack_seq4(H.S.data(), sum_len, r.seq.data(), r.seq.size());
+		sum_len += r.seq.size();
+		if (r.seq.empty()) continue;
+		std::vector<uint64_t> tmp((size_t)2 * (r.seq.size() / 2 + 64));
+		long n = wmo_sketch(r.seq.data(), (int)r.seq.size(), w, k, rid, bloom, tmp.data(), (long)tmp.size() / 2);
+		X.mz.insert(X.mz.end(), tmp.begin(), tmp.begin() + 2 * n);
+	}
+	set_name_order(&H);
+	return n_parts;
+}
+
+static int load_oracle_index(const char *ref_fn, const char *kmer_fn, int k, int w, OracleIndex &X)
+{
+	int rc = load_kmer_filter(kmer_fn, k, X);
+	if (rc == 0) rc = load_oracle_seqs(ref_fn, k, w, X.bloom, X);
+	return rc < 0 ? rc : 0;
+}
+
+typedef void (*MapBatchFn)(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads,
+                           std::vector<std::vector<wm_reg1_t>> &regs, std::vector<int> &rep_len, std::vector<int> &frag_gap, int n_threads, MapStats *stats);
+// how a batch is mapped on an oracle backend: the product's map_batch (hpc_backend.cpp maps through an HPC index instead)
+static MapBatchFn g_map_batch = map_batch;
+
+// The file driver's view (host_driver.h) of indexes served by oracle backends, one per part.  Under --cs / --MD every hit
+// mapped is formatted and its tag compared with what mm_gen_cs / mm_gen_MD give (gen_cs_or_MD).
+struct OracleParts : IndexParts {
+	std::vector<Backend*> be; std::vector<const wm_host_idx*> H;
+	wm_host_idx merged_H;           // the sequence table of all parts
+	std::vector<int32_t> f_mid_occ; // per part: mid_occ of the run's -f, -1 where the selection is refused
+	std::vector<int32_t> mid_occ;   // per part: the mid_occ it mapped with (-1: not mapped)
 	int n_gen_mismatch = 0;
-	if (sam) { write_sam_hdr(line, &H, "2.03", 0); fwrite(line.data(), 1, line.size(), out); }
-	for (size_t i = 0; i < reads.size(); ++i) { // the output step of the reference (src/map.c:1189-1206)
-		for (size_t j = 0; j < regs[i].size(); ++j) {
-			if ((mo.flag & WM_F_NO_PRINT_2ND) && regs[i][j].id != regs[i][j].parent) continue;
-			if (sam) write_sam(line, &H, reads[i], (int)j, (int)regs[i].size(), regs[i].data(), mo.flag, rl[i], "");
-			else write_paf(line, &H, reads[i], &regs[i][j], mo.flag, rl[i]);
-			fwrite(line.data(), 1, line.size(), out); fputc('\n', out);
-			if (regs[i][j].p && (mo.flag & (WM_F_OUT_CS | WM_F_OUT_MD))) { // mm_gen_cs / mm_gen_MD must give the tag's text
-				const bool md = (mo.flag & WM_F_OUT_MD) != 0;
-				std::string g;
-				gen_cs_or_MD(g, &H, &regs[i][j], reads[i]->seq.data(), md, !(mo.flag & WM_F_OUT_CS_LONG));
+	void add(Backend *b, const wm_host_idx *h)
+	{
+		be.push_back(b), H.push_back(h), mid_occ.push_back(-1);
+		merged_H.k = h->k, merged_H.w = h->w, merged_H.flag = h->flag;
+		merged_H.name.insert(merged_H.name.end(), h->name.begin(), h->name.end());
+		merged_H.len.insert(merged_H.len.end(), h->len.begin(), h->len.end());
+	}
+	int n_parts() const override { return (int)H.size(); }
+	const wm_host_idx *part(int p) const override { return H[p]; }
+	const wm_host_idx *all() const override { return H.size() == 1 ? H[0] : &merged_H; }
+	bool part_opt(int p, const wm_mapopt_t *opt, wm_mapopt_t *o) override
+	{
+		*o = *opt;
+		if (opt->mid_occ_frac >= 0 && opt->mid_occ_frac < 1) { // -f: what mm_mapopt_update sets per part
+			if (p >= (int)f_mid_occ.size() || f_mid_occ[p] < 0) return false;
+			o->mid_occ = std::max(f_mid_occ[p], opt->min_mid_occ), o->mid_occ_frac = -1.0f;
+		}
+		mid_occ[p] = o->mid_occ;
+		return true;
+	}
+	void map(int p, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads, std::vector<std::vector<wm_reg1_t>> &regs,
+	         std::vector<int> &rl, int n_threads) override
+	{
+		std::vector<int> fg;
+		g_map_batch(be[p], H[p], opt, reads, regs, rl, fg, n_threads, 0);
+		if (!(opt->flag & (WM_F_OUT_CS | WM_F_OUT_MD))) return;
+		const bool md = (opt->flag & WM_F_OUT_MD) != 0;
+		std::string line, g;
+		for (size_t i = 0; i < reads.size(); ++i)
+			for (size_t j = 0; j < regs[i].size(); ++j) {
+				if (!regs[i][j].p) continue;
+				if (opt->flag & WM_F_OUT_SAM) write_sam(line, H[p], reads[i], (int)j, (int)regs[i].size(), regs[i].data(), opt->flag, rl[i], "");
+				else write_paf(line, H[p], reads[i], &regs[i][j], opt->flag, rl[i]);
+				gen_cs_or_MD(g, H[p], &regs[i][j], reads[i]->seq.data(), md, !(opt->flag & WM_F_OUT_CS_LONG));
 				const size_t at = line.find(md ? "\tMD:Z:" : "\tcs:Z:");
 				if (at == std::string::npos || line.compare(at + 6, g.size(), g) != 0 || (at + 6 + g.size() < line.size() && line[at + 6 + g.size()] != '\t')) ++n_gen_mismatch;
 			}
-		}
-		if (regs[i].empty() && ((mo.flag & WM_F_PAF_NO_HIT) || (sam && !(mo.flag & WM_F_SAM_HIT_ONLY)))) {
-			if (sam) write_sam(line, &H, reads[i], -1, 0, 0, mo.flag, rl[i], "");
-			else write_paf(line, &H, reads[i], 0, mo.flag, rl[i]);
-			fwrite(line.data(), 1, line.size(), out); fputc('\n', out);
-		}
-		for (auto &rr : regs[i]) free(rr.p);
 	}
-	fclose(out);
-	return n_gen_mismatch ? -100 - n_gen_mismatch : 0;
+	// the whole read file in one batch (the golden inputs are far below the mini-batch of mapopt_init), rank 0 of 1
+	int run(const wm_mapopt_t &mo, const char *reads_fn, const char *out_fn, int n_threads)
+	{
+		const int rc = map_file(*this, &mo, reads_fn, out_fn, "", n_threads, 0, 1, 0, INT64_MAX);
+		return n_gen_mismatch ? -100 - n_gen_mismatch : rc;
+	}
+};
+
+// Maps every read of `reads_fn` through `be` with the product's file driver and writes PAF or SAM to `out_fn`
+static int map_file_on(Backend *be, const wm_host_idx &H, const wm_mapopt_t &mo, const char *reads_fn, const char *out_fn, int n_threads)
+{
+	OracleParts ix;
+	ix.add(be, &H);
+	return ix.run(mo, reads_fn, out_fn, n_threads);
 }
 
 static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *preset, const char *reads_fn, const char *out_fn, int n_threads, int sam, int64_t extra_flags = 0)
@@ -265,7 +312,7 @@ static int map_file_impl(const char *ref_fn, const char *kmer_fn, const char *pr
 	if ((rc = load_oracle_index(ref_fn, kmer_fn, io.k, io.w, X)) < 0) return rc;
 	CpuBackend be;
 	be.hidx = &X.H; be.bloom = X.bloom; be.idx = wmo_idx_build(X.mz.data(), (long)X.mz.size() / 2);
-	rc = map_reads_to(&be, X.H, mo, reads_fn, out_fn, n_threads, sam);
+	rc = map_file_on(&be, X.H, mo, reads_fn, out_fn, n_threads);
 	wmo_idx_free(be.idx);
 	return rc;
 }
@@ -291,10 +338,9 @@ extern "C" int wmt_map_file_sam(const char *ref_fn, const char *kmer_fn, const c
 // tuning aid: the orchestration's phase timers (WM_SUBTIMING=1 adds the per-task breakdown)
 extern "C" void wmt_dump_timers(void) { wmh::g_timers.dump(stderr); wmh::g_timers.reset(); }
 
-// unit hook: the index builder's parallel (hash, position) sort on an interleaved x,y array
-#include "../../winnowmap_b200/csrc/host_index.h"
 // unit hook: the index builder's 4-bit packing of a sequence placed at base offset o0 (S: zeroed words)
 extern "C" void wmt_pack_seq4(uint32_t *S, uint64_t o0, const char *seq, uint64_t L) { wmh::pack_seq4(S, o0, seq, L); }
+// unit hook: the index builder's parallel (hash, position) sort on an interleaved x,y array
 extern "C" void wmt_sort_index_pairs(uint64_t *xy, int64_t n, int n_threads)
 {
 	std::vector<wm_pair_t> a((size_t)n);

@@ -18,11 +18,10 @@ extern "C" int wmt_map_file_overlap(const char *ref_fn, const char *kmer_fn, con
 	OracleIndex X;
 	int rc = load_oracle_index(ref_fn, kmer_fn, io.k, io.w, X);
 	if (rc < 0) return rc;
-	set_name_order(&X.H);
 	OverlapCpuBackend be;
 	be.flag = mo.flag;
 	be.hidx = &X.H; be.bloom = X.bloom; be.idx = wmo_idx_build(X.mz.data(), (long)X.mz.size() / 2);
-	rc = map_reads_to(&be, X.H, mo, reads_fn, out_fn, n_threads, out_mode == 2);
+	rc = map_file_on(&be, X.H, mo, reads_fn, out_fn, n_threads);
 	wmo_idx_free(be.idx);
 	return rc;
 }

@@ -19,7 +19,6 @@ extern "C" int wmt_tee_overlap_seed_chain(const char *ref_fn, int k, int w, int 
 	TeeRun R;
 	int rc = R.init(ref_fn, 0, k, w, 0, dev_kind == 0 ? 0 : 1, 0, 0);
 	if (rc < 0) return rc;
-	set_name_order(&R.X.H);
 	OverlapCpuBackend ora, ora2;
 	for (OverlapCpuBackend *o : {&ora, &ora2}) o->flag = flag, o->hidx = &R.X.H, o->bloom = R.X.bloom, o->idx = R.cpu_e.idx;
 	R.tee.ora = &ora, R.tee.fetcher = &ora;

@@ -378,7 +378,7 @@ extern "C" int wmt_tee_map_file(const char *ref_fn, const char *kmer_fn, const c
 	if (rc < 0) return rc;
 	TeeRun R;
 	if ((rc = R.init(ref_fn, kmer_fn, io.k, io.w, hpc, dev_kind, mutation, budget)) < 0) return rc;
-	rc = map_reads_to(&R.tee, R.X.H, mo, reads_fn, out_fn, n_threads, 0);
+	rc = map_file_on(&R.tee, R.X.H, mo, reads_fn, out_fn, n_threads);
 	if (R.finish(report_fn) < 0) return -6;
 	return rc;
 }

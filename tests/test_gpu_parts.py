@@ -2,8 +2,6 @@
 reference's goldens (tests/golden/parts_*, made by tools/make_golden.py --parts), the per-part mid_occ the device selection
 gives (csrc/occ_select.cu) against the reference's and the plain-C oracle's, and the borrowed per-part handles."""
 import ctypes as C
-import gzip
-import hashlib
 import json
 import os
 import sys
@@ -14,7 +12,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tools"), os.path.join(ROOT, "tests")]
 import make_golden  # noqa: E402
-from test_parts_host import cal_max_occ  # noqa: E402
+from test_parts_host import cal_max_occ, check_output as _check, first_diff as _first_diff, golden as _golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 MAN = json.load(open(os.path.join(ROOT, "tests", "golden", "parts_manifest.json")))
@@ -51,18 +49,6 @@ def _lib():
     return L
 
 
-def _golden(name, suffix=".paf.gz"):
-    return gzip.open(os.path.join(ROOT, "tests", "golden", name + suffix)).read()
-
-
-def _first_diff(a, b):
-    la, lb = a.split(b"\n"), b.split(b"\n")
-    for i, (x, y) in enumerate(zip(la, lb)):
-        if x != y:
-            return f"line {i}: exp {x[:200]!r} got {y[:200]!r}"
-    return f"line count {len(la)} vs {len(lb)}"
-
-
 def _inputs(name, tmp_path):
     m = CASES[name]
     ref, reads, wfile = make_golden.make_parts_inputs(m["inputs"], str(tmp_path))
@@ -74,18 +60,6 @@ def _inputs(name, tmp_path):
 def _mapper(name, ref, wfile, **kw):
     from winnowmap_b200.mapper import Mapper
     return Mapper(ref, wfile, **dict(CASES[name]["lib"], **kw))
-
-
-def _check(name, got):
-    if CASES[name]["lib"].get("sam"):
-        got = make_golden.sam_without_pg(got)
-        if hashlib.md5(got).hexdigest() != CASES[name]["sam_md5"]:
-            exp, got = _golden(name, ".sam.stripped.gz"), make_golden.sam_strip_seq(got)
-            assert got == exp, _first_diff(exp, got)
-            pytest.fail("SEQ/QUAL differ")
-    else:
-        exp = _golden(name)
-        assert got == exp, _first_diff(exp, got)
 
 
 def _map(name, tmp_path, mapper_kw=None, **kw):

@@ -2,6 +2,7 @@
 reference's own (oracle/ref_harness_hpc.cpp), and the bit functions of the device's compaction front end (csrc/hpc.cuh)
 against a byte-per-base restatement."""
 import ctypes as C
+import glob
 import gzip
 import json
 import os
@@ -100,7 +101,7 @@ def hostsim(tmp_path_factory):
     so = str(tmp_path_factory.mktemp("hpc_hostsim") / "libwm_hostsim_hpc.so")
     subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-fopenmp", "-ffp-contract=off",
                            f"-I{os.environ.get('CUDA_HOME', '/usr/local/cuda')}/include", os.path.join(d, "hpc_backend.cpp"),
-                           os.path.join(d, "kernel_emul.cpp")] + [os.path.join(cs, f) for f in ("host_map.cpp", "host_align.cpp", "host_glue.cpp", "host_io.cpp", "host_format.cpp")] +
+                           os.path.join(d, "kernel_emul.cpp")] + sorted(glob.glob(os.path.join(cs, "host_*.cpp"))) +
                           ["-x", "c", os.path.join(ROOT, "oracle", "wm_oracle.c"), os.path.join(ROOT, "oracle", "wm_oracle_hpc.c"),
                            "-o", so, "-lz", "-lm", "-lpthread"], stderr=subprocess.DEVNULL)
     L = C.CDLL(so)

@@ -4,6 +4,7 @@ The product's host orchestration runs on the oracle backend with the seed filter
 (tests/hostsim/overlap_backend.cpp) and must reproduce the reference's goldens (tests/golden/overlap_*, made by
 tools/make_golden.py --overlap) byte for byte.  The name-rank reduction the device filter uses is checked against strcmp."""
 import ctypes as C
+import glob
 import gzip
 import hashlib
 import json
@@ -42,7 +43,7 @@ def overlap_sim(tmp_path_factory):
     cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
     subprocess.check_call(["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-fopenmp", "-ffp-contract=off", f"-I{cuda}/include",
                            os.path.join(d, "overlap_backend.cpp"), os.path.join(d, "kernel_emul.cpp")]
-                          + [os.path.join(cs, f) for f in ("host_map.cpp", "host_align.cpp", "host_glue.cpp", "host_io.cpp", "host_format.cpp")]
+                          + sorted(glob.glob(os.path.join(cs, "host_*.cpp")))
                           + ["-x", "c", os.path.join(ROOT, "oracle", "wm_oracle.c"), "-o", so, "-lz", "-lm", "-lpthread"])
     L = C.CDLL(so)
     L.wmt_map_file_overlap.argtypes = [C.c_char_p] * 5 + [C.c_int, C.c_int, C.c_int64]

@@ -1,7 +1,10 @@
-"""Index parts (-I) and the -f occurrence threshold on the host, no GPU: the library's part plan against the per-part
-sequence counts the reference printed (tests/golden/parts_manifest.json), and the plain-C restatement of
-mm_idx_cal_max_occ (oracle/wm_oracle_occ.c) against the reference's own function on every part of the parts inputs."""
+"""Index parts (-I), --split-prefix and the -f occurrence threshold on the host, no GPU: the library's part plan against the
+per-part sequence counts the reference printed (tests/golden/parts_manifest.json), the plain-C restatement of
+mm_idx_cal_max_occ (oracle/wm_oracle_occ.c) against the reference's own function on every part of the parts inputs, and
+the product's file driver (csrc/host_driver.cpp) on oracle backends, one per part, against the reference's parts goldens."""
 import ctypes as C
+import gzip
+import hashlib
 import json
 import os
 import subprocess
@@ -17,6 +20,9 @@ import make_golden  # noqa: E402
 
 MAN = json.load(open(os.path.join(ROOT, "tests", "golden", "parts_manifest.json")))
 _occ = None
+# the goldens the oracle-backed pipeline reproduces (-H and -X have harnesses of their own)
+HOST_CASES = ["parts_ont_c", "parts_ont_a", "parts_ont_c_split", "parts_ont_a_split", "parts_single_split_c", "parts_single_split_a",
+              "parts_tandem_f0002", "parts_tandem_f0002_I", "parts_tandem_f01", "parts_tandem_f01_I_split"]
 
 
 def occ_oracle():
@@ -100,3 +106,54 @@ def test_cal_max_occ_restatement_edges():
     assert cal_max_occ(c, 0.99) == 2             # rank (uint32)(0.01 * 6) = 0
     assert cal_max_occ(c, 0.25) == 10            # rank 4
     assert cal_max_occ(c, 0.1) == (1 << 20) + 1  # rank 5 = n - 1
+
+
+def golden(name, suffix=".paf.gz"):
+    return gzip.open(os.path.join(ROOT, "tests", "golden", name + suffix)).read()
+
+
+def first_diff(a, b):
+    la, lb = a.split(b"\n"), b.split(b"\n")
+    for i, (x, y) in enumerate(zip(la, lb)):
+        if x != y:
+            return f"line {i}: exp {x[:200]!r} got {y[:200]!r}"
+    return f"line count {len(la)} vs {len(lb)}"
+
+
+def check_output(name, got):
+    """got is the golden of parts case `name`: PAF byte for byte, SAM but for the @PG line."""
+    if MAN["cases"][name]["lib"].get("sam"):
+        got = make_golden.sam_without_pg(got)
+        if hashlib.md5(got).hexdigest() != MAN["cases"][name]["sam_md5"]:
+            exp, got = golden(name, ".sam.stripped.gz"), make_golden.sam_strip_seq(got)
+            assert got == exp, first_diff(exp, got)
+            pytest.fail("SEQ/QUAL differ")
+    else:
+        exp = golden(name)
+        assert got == exp, first_diff(exp, got)
+
+
+@pytest.fixture(scope="module")
+def hostsim():
+    d = os.path.join(ROOT, "tests", "hostsim")
+    subprocess.check_call([os.path.join(d, "build.sh")], stderr=subprocess.DEVNULL)
+    L = C.CDLL(os.path.join(d, "libwm_hostsim.so"))
+    L.wmt_map_file_parts.argtypes = [C.c_char_p] * 5 + [C.c_int, C.c_int, C.c_uint64, C.c_int, C.c_float, C.POINTER(C.c_int32), C.c_int]
+    return L
+
+
+@pytest.mark.parametrize("name", HOST_CASES)
+def test_parts_pipeline_matches_reference(hostsim, name, tmp_path):
+    """The file driver on oracle backends: part-major and merged output, the SAM headers of both (no @SQ part-major, the
+    merge's @SQ lines after the header's) and -f resolved per part, with the mid_occ each part mapped with."""
+    m = MAN["cases"][name]
+    o = m["lib"]
+    ref, reads, wfile = make_golden.make_parts_inputs(m["inputs"], str(tmp_path))
+    assert make_golden.md5(ref) == m["ref_md5"] and make_golden.md5(reads) == m["reads_md5"], "synthetic input generator drifted"
+    out = str(tmp_path / "out")
+    mid_occ = (C.c_int32 * 16)()
+    n = hostsim.wmt_map_file_parts(ref.encode(), wfile.encode() if wfile else None, o["preset"].encode(), reads.encode(), out.encode(), 8,
+                                   int(bool(o.get("sam"))), o.get("part_bases", 0), int(bool(o.get("split"))), o.get("mid_occ_frac", -1.0), mid_occ, 16)
+    assert n == len(m["n_seq"])
+    assert list(mid_occ[:n]) == m["mid_occ"]
+    check_output(name, open(out, "rb").read())

@@ -1,12 +1,11 @@
-// C-ABI of the drop-in boundary (include/winnowmap_b200.h): index upload / construction, batch mapping
-// (the replacement of kt_for(worker_for), reference src/map.c:1162-1165) and the file-level driver that mirrors
-// mm_map_file (src/map.c:1244-1276) for PAF output.
+// C-ABI of the drop-in boundary (include/winnowmap_b200.h): the CUDA context, its lanes, index upload / construction and
+// batch mapping (the replacement of kt_for(worker_for), reference src/map.c:1162-1165).  The file-level driver
+// (host_driver.cpp) runs over a context through CtxParts.
 #include <stddef.h>
 #include <string.h>
 #include <algorithm>
 #include <atomic>
 #include <chrono>
-#include <condition_variable>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -17,6 +16,7 @@
 #include "topfreq.cuh"
 #include "occ_select.cuh"
 #include "gpu_backend.h"
+#include "host_driver.h"
 #include "host_io.h"
 #include "host_index.h"
 #include "host_timers.h"
@@ -88,9 +88,8 @@ static void ensure_lanes(wm_gpu_ctx_s *c, int n_threads)
 }
 
 static void map_lanes(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads, std::vector<std::vector<wm_reg1_t>> &regs,
-                      std::vector<int> &rl, std::vector<int> &fg, int n_threads, bool resident)
+                      std::vector<int> &rl, std::vector<int> &fg, int n_threads)
 {
-	(void)resident;
 	wm_gpu_ctx_s *r = root_of(c);
 	ensure_lanes(r, n_threads);
 	for (Backend *lane : r->lanes) gpu_backend_bind(lane, c->be); // a part of a multi-part index maps with the root's lanes
@@ -242,27 +241,8 @@ struct ref_pools {
 	}
 };
 
-// Where mm_idx_gen ends an index part (src/index.c:289-297 and :660-671, src/bseq.c:80-119): a part is read in mini-batches
-// of min(mini_batch_size, batch_size) bases, each mini-batch whole sequences until it holds at least that many bases, and
-// no further mini-batch is started once the part holds more than batch_size bases.
-struct PartCutter {
-	uint64_t batch, mb, part_sum = 0, mb_sum = 0;
-	bool open = false; // a mini-batch is being filled
-	int part = -1;
-	PartCutter(uint64_t batch_size, int mini_batch_size) : batch(batch_size), mb((uint64_t)mini_batch_size < batch_size ? (uint64_t)mini_batch_size : batch_size) {}
-	int next(uint64_t len) // the part of the next sequence
-	{
-		if (!open) {
-			if (part < 0 || part_sum > batch) ++part, part_sum = 0;
-			open = true, mb_sum = 0;
-		}
-		mb_sum += len;
-		if (mb_sum >= mb) part_sum += mb_sum, open = false;
-		return part;
-	}
-};
-
-// H (if not null) gets one sequence table per part: rid and offset restart at 0 in every part
+// The reference is cut into index parts by PartCutter (host_driver.h); H (if not null) gets one sequence table per part:
+// rid and offset restart at 0 in every part
 static bool read_ref_pools(const char *ref_fn, std::vector<wm_host_idx> *H, uint64_t batch_size, int mini_batch_size, ref_pools &P)
 {
 	SeqReader rd;
@@ -576,41 +556,22 @@ extern "C" int wm_abi_layout(int64_t *out, int cap)
 // The parts of a context in order: its own index for a single one
 static std::vector<wm_gpu_ctx_s*> parts_of(wm_gpu_ctx_s *c) { return is_multi(c) ? c->parts : std::vector<wm_gpu_ctx_s*>(1, c); }
 
-// --split-prefix: every read mapped against every part, then merge_hits (src/map.c:1050-1105) in memory: the regs of the
-// parts concatenated in part order, rid shifted by the sequences of the earlier parts, then mm_hit_sort, mm_set_parent,
-// mm_select_sub and mm_set_sam_pri (not under MM_F_ALL_CHAINS) and mm_set_mapq with the largest rep_len of the parts.
-static bool map_merged(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads, std::vector<std::vector<wm_reg1_t>> &regs, int n_threads)
-{
-	const std::vector<wm_gpu_ctx_s*> parts = parts_of(c);
-	const int n = (int)reads.size();
-	regs.assign(n, std::vector<wm_reg1_t>());
-	std::vector<int> rep_len(n, 0);
-	int32_t rid_shift = 0;
-	for (wm_gpu_ctx_s *p : parts) {
-		wm_mapopt_t o;
-		if (!part_opt(p, opt, &o)) return false;
-		std::vector<std::vector<wm_reg1_t>> r; std::vector<int> rl, fg;
-		map_lanes(p, &o, reads, r, rl, fg, n_threads, false);
-		for (int i = 0; i < n; ++i) {
-			for (auto &x : r[i]) { x.rid += rid_shift; regs[i].push_back(x); }
-			rep_len[i] = std::max(rep_len[i], rl[i]);
-		}
-		rid_shift += (int32_t)p->hidx.name.size();
+// The file driver's view of a context (host_driver.h): its parts, each mapped with the root's lanes, and -f resolved per
+// part by part_opt with the occurrence cache
+struct CtxParts : IndexParts {
+	wm_gpu_ctx_s *c; std::vector<wm_gpu_ctx_s*> parts;
+	explicit CtxParts(wm_gpu_ctx_s *c) : c(c), parts(parts_of(c)) {}
+	int n_parts() const override { return (int)parts.size(); }
+	const wm_host_idx *part(int p) const override { return &parts[p]->hidx; }
+	const wm_host_idx *all() const override { return &c->hidx; }
+	bool part_opt(int p, const wm_mapopt_t *opt, wm_mapopt_t *o) override { return ::part_opt(parts[p], opt, o); }
+	void map(int p, const wm_mapopt_t *opt, const std::vector<const wm_read*> &reads, std::vector<std::vector<wm_reg1_t>> &regs,
+	         std::vector<int> &rep_len, int n_threads) override
+	{
+		std::vector<int> fg;
+		map_lanes(parts[p], opt, reads, regs, rep_len, fg, n_threads);
 	}
-	const int k = c->hidx.k;
-	#pragma omp parallel for schedule(dynamic, 16) num_threads(n_threads > 0 ? n_threads : 1)
-	for (int i = 0; i < n; ++i) {
-		std::vector<wm_reg1_t> &v = regs[i];
-		hit_sort(v, opt->alt_drop);
-		set_parent(opt->mask_level, opt->mask_len, (int)v.size(), v.data(), opt->a * 2 + opt->b, (int)(opt->flag & WM_F_HARD_MLEVEL), opt->alt_drop);
-		if (!(opt->flag & WM_F_ALL_CHAINS)) {
-			select_sub(opt->pri_ratio, k * 2, opt->best_n, v);
-			set_sam_pri((int)v.size(), v.data());
-		}
-		set_mapq(v, opt->min_chain_score, opt->a, rep_len[i], 0);
-	}
-	return true;
-}
+};
 
 // The GPU replacement of kt_for(n_threads, worker_for, ...) (src/map.c:1164): fills n_reg/reg/rep_len/frag_gap of
 // every sequence exactly as worker_for does (:1025-1034).  reg[i] and each reg[i][j].p are malloc()ed; the caller
@@ -634,12 +595,13 @@ extern "C" int wm_gpu_map_batch(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, int n_s
 			fprintf(stderr, "[ERROR] wm_gpu_map_batch: a multi-part index maps part by part (wm_idx_part) unless split_prefix asks for merged hits\n");
 			return -1;
 		}
-		if (!map_merged(c, opt, reads, regs, n_threads)) return -1;
+		CtxParts ix(c);
+		if (!map_merged(ix, opt, reads, regs, n_threads)) return -1;
 		rl.assign(n_seq, 0), fg.assign(n_seq, 0);
 	} else {
 		wm_mapopt_t o;
 		if (!part_opt(c, opt, &o)) return -1;
-		map_lanes(c, &o, reads, regs, rl, fg, n_threads, false);
+		map_lanes(c, &o, reads, regs, rl, fg, n_threads);
 	}
 	for (int i = 0; i < n_seq; ++i) {
 		n_reg[i] = (int32_t)regs[i].size();
@@ -670,155 +632,14 @@ extern "C" wm_reg1_t *wm_map(wm_gpu_ctx_s *c, int l_seq, const char *seq, int *n
 	return reg;
 }
 
-// mm_map_file for PAF output.  Reads are taken in the reference's mini-batches (src/bseq.c:80-119), sorted by
-// length descending inside a batch (src/map.c:1124-1143) and printed in that order (:1173-1208).  With world > 1
-// this process maps and prints only the reads whose position in the sorted batch is rank mod world; every output
-// line is preceded by "<batch>\t<position>\t" when tag_order != 0 so that the shards can be merged back.
-// One pass over the read file: c is one index (mapped and written as mm_map_file does), or, with `merged`, the context whose
-// parts are all mapped and merged per read (map_merged), written with the sequence table of all parts.
-static int map_file_pass(wm_gpu_ctx_s *c, const wm_mapopt_t *opt_in, const char *reads_fn, FILE *out, int n_threads, int rank, int world,
-                         int tag_order, int64_t max_batch_bases, bool merged)
-{
-	SeqReader rd;
-	if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
-	wm_mapopt_t opt_part;
-	if (!merged && !part_opt(c, opt_in, &opt_part)) return -1;
-	const wm_mapopt_t *opt = merged ? opt_in : &opt_part;
-	const int64_t chunk = opt->mini_batch_size;
-	bool failed = false;
-	// The three steps of the reference's pipeline (src/map.c:1107-1224: read, map, write) run on three threads with
-	// one mini-batch of slack between them: the next batch is parsed and the previous one formatted while the GPU maps.
-	struct FileBatch {
-		int64_t no;
-		std::vector<wm_read> reads;
-		std::vector<const wm_read*> mine; std::vector<int> mine_pos;          // this rank's reads, in output order
-		std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl;        // aligned with `mine`
-	};
-	struct Slot { // a one-element hand-over queue
-		std::mutex mu; std::condition_variable cv; FileBatch *item = 0; bool closed = false;
-		void put(FileBatch *b) { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return item == 0; }); item = b; cv.notify_all(); }
-		void close() { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return item == 0; }); closed = true; cv.notify_all(); }
-		FileBatch *get() { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return item != 0 || closed; }); FileBatch *b = item; item = 0; cv.notify_all(); return b; }
-	} q_in, q_out;
-	std::thread reader([&]() {
-		int64_t batch_no = 0;
-		for (;;) {
-			FileBatch *b = new FileBatch();
-			int64_t size = 0;
-			wm_read r;
-			const bool with_qual = (opt->flag & WM_F_OUT_SAM) && !(opt->flag & WM_F_NO_QUAL); // src/map.c:1112
-			while (rd.next(r)) {
-				size += (int64_t)r.seq.size();
-				if (!with_qual) r.qual.clear();
-				b->reads.push_back(r);
-				if (size >= chunk) break;
-			}
-			if (b->reads.empty()) { delete b; break; }
-			b->no = batch_no++;
-			q_in.put(b);
-		}
-		q_in.close();
-	});
-	std::thread writer([&]() {
-		std::vector<std::string> lines;
-		for (;;) {
-			FileBatch *b = q_out.get();
-			if (!b) break;
-			const int n = (int)b->mine.size();
-			lines.assign(n, std::string());
-			#pragma omp parallel num_threads(n_threads > 8 ? 8 : (n_threads > 0 ? n_threads : 1))
-			{
-				std::string line; char tag[64];
-				#pragma omp for schedule(dynamic, 16)
-				for (int i = 0; i < n; ++i) {
-					const wm_read *t = b->mine[i];
-					std::string &dst = lines[i];
-					const bool sam = (opt->flag & WM_F_OUT_SAM) != 0;
-					auto emit = [&](int j) { // hit j of the read, or the empty record (j < 0), src/map.c:1189-1206
-						if (sam) write_sam(line, &c->hidx, t, j, (int)b->regs[i].size(), b->regs[i].data(), opt->flag, b->rl[i], "");
-						else write_paf(line, &c->hidx, t, j >= 0 ? &b->regs[i][j] : 0, opt->flag, b->rl[i]);
-						if (tag_order) { snprintf(tag, sizeof(tag), "%lld\t%d\t", (long long)b->no, b->mine_pos[i]); dst += tag; }
-						dst += line; dst += '\n';
-					};
-					if (!b->regs[i].empty()) {
-						for (size_t j = 0; j < b->regs[i].size(); ++j) {
-							const wm_reg1_t *rr = &b->regs[i][j];
-							if ((opt->flag & WM_F_NO_PRINT_2ND) && rr->id != rr->parent) continue;
-							emit((int)j);
-						}
-					} else if ((opt->flag & WM_F_PAF_NO_HIT) || (sam && !(opt->flag & WM_F_SAM_HIT_ONLY))) emit(-1);
-					for (auto &rr : b->regs[i]) free(rr.p);
-				}
-			}
-			for (int i = 0; i < n; ++i) fwrite(lines[i].data(), 1, lines[i].size(), out);
-			delete b;
-		}
-	});
-	for (;;) {
-		FileBatch *b = q_in.get();
-		if (!b) break;
-		// longer reads first; ties by larger input index first (std::greater on (len, index), src/map.c:1129)
-		std::vector<std::pair<int, int>> ord;
-		for (size_t i = 0; i < b->reads.size(); ++i) ord.emplace_back((int)b->reads[i].seq.size(), (int)i);
-		std::sort(ord.begin(), ord.end(), std::greater<std::pair<int, int>>());
-		for (size_t p = 0; p < ord.size(); ++p)
-			if ((int)(p % (size_t)world) == rank) { b->mine.push_back(&b->reads[ord[p].second]); b->mine_pos.push_back((int)p); }
-		b->regs.resize(b->mine.size()); b->rl.assign(b->mine.size(), 0);
-		// internal sub-batches bound device memory; results do not depend on how reads are grouped
-		size_t s0 = 0;
-		while (s0 < b->mine.size()) {
-			size_t s1 = s0; int64_t nb = 0;
-			while (s1 < b->mine.size() && (s1 == s0 || nb + (int64_t)b->mine[s1]->seq.size() <= max_batch_bases)) nb += (int64_t)b->mine[s1]->seq.size(), ++s1;
-			std::vector<const wm_read*> sub(b->mine.begin() + s0, b->mine.begin() + s1);
-			std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-			if (merged) { // the merge pass leaves rep_len 0 in what it prints (src/map.c:1050-1105 does not set it)
-				if (!failed && !map_merged(c, opt, sub, regs, n_threads)) failed = true;
-				if (failed) regs.assign(sub.size(), std::vector<wm_reg1_t>());
-				rl.assign(sub.size(), 0);
-			} else map_lanes(c, opt, sub, regs, rl, fg, n_threads, false);
-			for (size_t i = 0; i < sub.size(); ++i) { b->regs[s0 + i].swap(regs[i]); b->rl[s0 + i] = rl[i]; }
-			s0 = s1;
-		}
-		q_out.put(b);
-	}
-	q_out.close();
-	reader.join(); writer.join();
-	return failed ? -1 : 0;
-}
-
-// Without split_prefix a multi-part index is mapped part by part and written part-major, as the reference's loop over the
-// parts does (src/main.c:384-424); the SAM header then has no @SQ line (mm_write_sam_hdr(0, ...), :391-398).  With
-// split_prefix the parts' hits are merged per read in one pass (mm_split_merge, src/map.c:1278-1321), also for a single
-// index: its @SQ lines then come twice, the normal header's and the merge's, as the reference prints them.  The reference
-// goes through temporary files <prefix>.NNNN.tmp; here the merge runs in memory and no file is written.
+// mm_map_file (src/map.c:1244-1276) over the parts of c: the driver of host_driver.cpp with the context's lanes
 extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, int n_threads, int rank, int world,
                            int tag_order, int64_t max_batch_bases)
 {
 	require_device("wm_map_file");
-	const bool merged = opt->split_prefix != 0;
-	if (is_multi(c) && !merged && world > 1) {
-		fprintf(stderr, "[ERROR] wm_map_file: a multi-part index without split_prefix is written part-major, which does not shard over ranks\n");
-		return -1;
-	}
-	{ // the read file is checked before the output is created
-		SeqReader rd;
-		if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
-	}
-	FILE *out = out_fn && strcmp(out_fn, "-") ? fopen(out_fn, "wb") : stdout;
-	if (!out) return -1;
 	const double t0 = now_s();
-	if ((opt->flag & WM_F_OUT_SAM) && rank == 0 && !tag_order) { // mm_write_sam_hdr (src/main.c:391-398); the merge's @SQ lines follow (src/map.c:1304-1306)
-		std::string h;
-		wm_host_idx none;
-		write_sam_hdr(h, is_multi(c) ? &none : &c->hidx, "2.03", c->sam_cl.c_str());
-		if (merged)
-			for (size_t i = 0; i < c->hidx.name.size(); ++i) { h += "@SQ\tSN:"; h += c->hidx.name[i]; h += "\tLN:"; h += std::to_string(c->hidx.len[i]); h += '\n'; }
-		fwrite(h.data(), 1, h.size(), out);
-	}
-	int rc = 0;
-	if (merged) rc = map_file_pass(c, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases, true);
-	else for (wm_gpu_ctx_s *p : parts_of(c)) if (rc == 0) rc = map_file_pass(p, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases, false);
-	if (out != stdout) fclose(out); else fflush(out);
+	CtxParts ix(c);
+	const int rc = map_file(ix, opt, reads_fn, out_fn, c->sam_cl.c_str(), n_threads, rank, world, tag_order, max_batch_bases);
 	c->t_map += now_s() - t0;
 	return rc;
 }
@@ -954,7 +775,7 @@ extern "C" int wm_bench_map_resident(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, in
 		std::vector<const wm_read*> reads(g1 - g0);
 		for (int i = g0; i < g1; ++i) reads[i - g0] = &c->resident[i];
 		std::vector<std::vector<wm_reg1_t>> regs; std::vector<int> rl, fg;
-		map_lanes(c, opt, reads, regs, rl, fg, n_threads, true);
+		map_lanes(c, opt, reads, regs, rl, fg, n_threads);
 		for (int i = g0; i < g1; ++i) { c->res_regs[i].swap(regs[i - g0]); c->res_rl[i] = rl[i - g0]; }
 	}
 	WM_CUDA_CHECK(cudaEventRecord(e1, 0));
@@ -963,24 +784,6 @@ extern "C" int wm_bench_map_resident(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, in
 	WM_CUDA_CHECK(cudaEventElapsedTime(&f, e0, e1));
 	*ms = f;
 	return 0;
-}
-
-// One read's output lines (PAF, or SAM when opt->flag says so), as the output step of the reference prints them (src/map.c:1189-1206)
-static void format_read(std::string &dst, const wm_host_idx *mi, const wm_mapopt_t *opt, const wm_read *t, int n_reg, const wm_reg1_t *regs, int rep_len)
-{
-	std::string line;
-	const bool sam = (opt->flag & WM_F_OUT_SAM) != 0;
-	auto emit = [&](int j) {
-		if (sam) write_sam(line, mi, t, j, n_reg, regs, opt->flag, rep_len, "");
-		else write_paf(line, mi, t, j >= 0 ? &regs[j] : 0, opt->flag, rep_len);
-		dst += line; dst += '\n';
-	};
-	if (n_reg > 0) {
-		for (int j = 0; j < n_reg; ++j) {
-			if ((opt->flag & WM_F_NO_PRINT_2ND) && regs[j].id != regs[j].parent) continue;
-			emit(j);
-		}
-	} else if ((opt->flag & WM_F_PAF_NO_HIT) || (sam && !(opt->flag & WM_F_SAM_HIT_ONLY))) emit(-1);
 }
 
 // bench: the records of the last resident pass, formatted for the first n_first reads in input order (parity check of the timed path)
@@ -992,7 +795,7 @@ extern "C" int wm_bench_write(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, int n_fir
 	std::string buf;
 	for (int i = 0; i < n; ++i) {
 		buf.clear();
-		format_read(buf, &c->hidx, opt, &c->resident[i], (int)c->res_regs[i].size(), c->res_regs[i].data(), c->res_rl[i]);
+		format_read(buf, &c->hidx, opt->flag, &c->resident[i], (int)c->res_regs[i].size(), c->res_regs[i].data(), c->res_rl[i]);
 		fwrite(buf.data(), 1, buf.size(), out);
 	}
 	fclose(out);
@@ -1011,7 +814,7 @@ extern "C" int wm_format_batch(const wm_gpu_ctx_s *c, const wm_mapopt_t *opt, in
 		t.name = names && names[i] ? names[i] : "";
 		t.seq.assign(seqs[i], lens[i]);
 		buf.clear();
-		format_read(buf, &c->hidx, opt, &t, n_reg[i], reg[i], rep_len[i]);
+		format_read(buf, &c->hidx, opt->flag, &t, n_reg[i], reg[i], rep_len[i]);
 		fwrite(buf.data(), 1, buf.size(), out);
 	}
 	fclose(out);
