@@ -12,6 +12,7 @@
 #define WM_HOST_EMUL 1
 
 namespace wm_emul {
+struct Cta;
 // The 32 lanes are fibers (ucontext) of one host thread, scheduled round-robin; a barrier is "yield until everybody
 // has arrived", so a warp-level operation costs a few context switches instead of an OS barrier.
 struct Warp {
@@ -20,8 +21,14 @@ struct Warp {
 	bool done[32];
 	int cur, arrived, gen;
 	uint64_t xchg[32];
-	void (*body)(int lane, void *arg); void *arg;
+	void (*body)(int lane, void *arg); void *arg; // (in a CTA, body receives the thread index 32 * id + lane)
+	// the rest is used by CTA runs only (run_cta): the CTA (0 for a lone warp of run_warp), the warp's index there, what each lane
+	// waits for (LANE_*), the warp's run count and, per polling lane, the run in which it polled, and the CTA event count at which
+	// the warp was found blocked (-1: runnable)
+	Cta *cta; int id, n_done;
+	int8_t state[32]; long long run, polled_in[32], blocked_at;
 };
+enum { LANE_RUN = 0, LANE_SYNC = 1, LANE_POLL = 2, LANE_BAR = 3 };
 extern thread_local Warp *warp;
 extern thread_local int lane;
 inline void yield_lane()
@@ -33,13 +40,19 @@ inline void yield_lane()
 	if (nxt == me) return;
 	w->cur = nxt;
 	swapcontext(&w->ctx[me], &w->ctx[nxt]);
-	lane = me; // (thread_local shared by all fibers)
+	warp = w, lane = me; // (thread_local shared by all fibers; in a CTA another warp may have run meanwhile)
 }
+void cta_sync_done(Warp *w); // kernel_emul.cpp: a warp-wide sync of w completed: the CTA's scheduler may run another warp
 inline void sync()
 {
 	Warp *w = warp;
 	const int gen = w->gen;
-	if (++w->arrived == 32) { w->arrived = 0; ++w->gen; return; }
+	if (++w->arrived == 32) {
+		w->arrived = 0; ++w->gen;
+		if (w->cta) cta_sync_done(w);
+		return;
+	}
+	if (w->cta) w->state[lane] = LANE_SYNC;
 	while (w->gen == gen) yield_lane();
 }
 template <typename T> inline T exchange(T v, int src_lane)
@@ -53,6 +66,36 @@ template <typename T> inline T exchange(T v, int src_lane)
 	return out;
 }
 void run_warp(void (*body)(int lane, void *arg), void *arg); // kernel_emul.cpp: runs body on 32 lockstep lanes
+
+// ---- a CTA of several software warps (kernel_emul.cpp: run_cta) ----
+// Lanes of a warp stay lockstep fibers.  Warps are switched only where a warp can stall on the hardware: when one of its warp-wide
+// syncs completes (ballot, shuffle, __syncwarp), at __syncthreads and at __nanosleep.  A warp is blocked when every unfinished lane
+// polls (__nanosleep) or waits at a sync or barrier; it becomes runnable again after an atomic operation, a barrier release or the
+// end of a warp (what lets a polling warp of the kernels go on), or when every warp is blocked: then all are tried once more, and
+// if no sync or barrier completes before they block again, the run stops with a deadlock.
+enum { SCHED_ROUND_ROBIN = 0, SCHED_RANDOM = 1, SCHED_LAGGARD = 2, SCHED_LEADER = 3 };
+enum { ATOM_ADD = 0, ATOM_OR = 1, ATOM_CAS = 2, ATOM_EXCH = 3 };
+struct Cta {
+	int n_warps; Warp *w;
+	// SCHED_ROUND_ROBIN: the next runnable warp after every completed sync; SCHED_RANDOM: a runnable warp drawn with rng;
+	// SCHED_LAGGARD: warp sched_warp runs only when every other warp is blocked; SCHED_LEADER: warp sched_warp runs whenever it can
+	int sched, sched_warp; uint64_t rng;
+	long long poll_bound;  // polls without a completed sync or barrier after which the run counts as deadlocked
+	// observer of the atomic operations (kind ATOM_*, the warp, the address, the old value, whether a CAS succeeded), may be 0; it
+	// returns whether a polling warp could be waiting for that operation (without an observer, every one that changes memory counts)
+	bool (*on_atomic)(void *user, int kind, int warp, const void *addr, unsigned long long old, bool ok); void *user;
+	// statistics and state
+	long long events, syncs, polls, polls_since_sync, sweeps, syncs_at_sweep, switches, bar_gen;
+	int bar_arrived, live_threads, deadlock;
+	ucontext_t main_ctx;
+};
+void cta_poll();    // __nanosleep of a lane in a CTA
+void cta_barrier(); // __syncthreads
+void cta_atomic(int kind, const void *addr, unsigned long long old, bool ok);
+// Runs body(tid, arg) on c->n_warps warps of 32 lanes; the caller sets the schedule fields, poll_bound and on_atomic of c.  Returns 0,
+// or -1 after a deadlock (c->deadlock = 1; the lanes are abandoned where they stood).
+int run_cta(Cta *c, void (*body)(int tid, void *arg), void *arg);
+inline void note_atomic(int kind, const void *addr, unsigned long long old, bool ok) { if (warp && warp->cta) cta_atomic(kind, addr, old, ok); }
 } // namespace wm_emul
 
 inline void __syncwarp(unsigned = 0xffffffffu) { wm_emul::sync(); }
@@ -60,10 +103,19 @@ template <typename T> inline T __shfl_sync(unsigned, T v, int src, int = 32) { r
 template <typename T> inline T __shfl_up_sync(unsigned, T v, unsigned d, int = 32)
 { const int src = wm_emul::lane - (int)d; const T r = wm_emul::exchange(v, src < 0 ? wm_emul::lane : src); return src < 0 ? v : r; }
 template <typename T> inline T __shfl_xor_sync(unsigned, T v, int m, int = 32) { return wm_emul::exchange(v, wm_emul::lane ^ m); }
-inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v)
+{ const unsigned long long o = __atomic_fetch_add(p, v, __ATOMIC_RELAXED); wm_emul::note_atomic(wm_emul::ATOM_ADD, p, o, true); return o; }
+inline int atomicAdd(int *p, int v) { const int o = __atomic_fetch_add(p, v, __ATOMIC_RELAXED); wm_emul::note_atomic(wm_emul::ATOM_ADD, p, (unsigned)o, true); return o; }
 inline int atomicMin(int *p, int v) { int o = *p; if (v < o) *p = v; return o; }
-inline unsigned atomicOr(unsigned *p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
+inline unsigned atomicOr(unsigned *p, unsigned v) { const unsigned o = __atomic_fetch_or(p, v, __ATOMIC_RELAXED); wm_emul::note_atomic(wm_emul::ATOM_OR, p, o, true); return o; }
+inline int atomicCAS(int *p, int cmp, int v) { const int o = *p; if (o == cmp) *p = v; wm_emul::note_atomic(wm_emul::ATOM_CAS, p, (unsigned)o, o == cmp); return o; }
+inline int atomicExch(int *p, int v) { const int o = *p; *p = v; wm_emul::note_atomic(wm_emul::ATOM_EXCH, p, (unsigned)o, true); return o; }
+// a lone warp (run_warp) has nobody to wait for: its polls only let the other lanes go on
+inline void __nanosleep(unsigned) { if (wm_emul::warp->cta) wm_emul::cta_poll(); else wm_emul::yield_lane(); }
+inline void __syncthreads() { if (wm_emul::warp->cta) wm_emul::cta_barrier(); else wm_emul::sync(); }
+// the emulation is sequentially consistent: fences and cache hints have nothing to do
+inline void __threadfence_block() {}
+template <typename T> inline T __ldcg(const T *p) { return *p; }
 
 // ---- integer SIMD-in-a-word intrinsics (CUDA math API semantics) ----
 inline uint32_t wm_emul_pack(int lo, int hi) { return ((uint32_t)lo & 0xffffu) | ((uint32_t)hi << 16); }

@@ -18,25 +18,28 @@
 namespace wm_emul {
 thread_local Warp *warp = 0; thread_local int lane = 0;
 static long long g_total_syncs = 0; // warp-wide synchronisation points executed so far (a proxy for dependent steps)
+static void cta_warp_finished(Warp *w);
 static void fiber_entry()
 {
 	Warp *w = warp;
 	const int me = w->cur;
 	lane = me;
-	w->body(me, w->arg);
+	w->body(w->cta ? 32 * w->id + me : me, w->arg);
 	w->done[me] = true;
+	++w->n_done;
 	// a finished lane never comes back: continue with another unfinished lane, or return to the caller
 	for (int k = 1; k <= 32; ++k) {
 		const int nxt = (me + k) & 31;
 		if (!w->done[nxt]) { w->cur = nxt; setcontext(&w->ctx[nxt]); }
 	}
+	if (w->cta) cta_warp_finished(w); // (does not return)
 	setcontext(&w->main_ctx);
 }
 void run_warp(void (*body)(int lane, void *arg), void *arg)
 {
 	Warp W;
 	memset(W.done, 0, sizeof(W.done));
-	W.cur = 0, W.arrived = 0, W.gen = 0, W.body = body, W.arg = arg;
+	W.cur = 0, W.arrived = 0, W.gen = 0, W.body = body, W.arg = arg, W.cta = 0, W.id = 0, W.n_done = 0;
 	const size_t stack_bytes = (size_t)1 << 18;
 	for (int l = 0; l < 32; ++l) {
 		W.stack[l] = (char*)malloc(stack_bytes);
@@ -50,6 +53,143 @@ void run_warp(void (*body)(int lane, void *arg), void *arg)
 	warp = saved;
 	g_total_syncs += W.gen;
 	for (int l = 0; l < 32; ++l) free(W.stack[l]);
+}
+
+// ---- CTA runs (cuda_emul.h: run_cta) ----
+static bool runnable(const Cta *c, const Warp *x) { return x->n_done < 32 && (x->blocked_at < 0 || x->blocked_at < c->events); }
+// every unfinished lane of w waits at a sync or barrier, or has polled since w last resumed
+static bool warp_blocked(const Warp *w)
+{
+	for (int l = 0; l < 32; ++l)
+		if (!w->done[l] && (w->state[l] == LANE_RUN || (w->state[l] == LANE_POLL && w->polled_in[l] != w->run))) return false;
+	return true;
+}
+static uint64_t next_rand(Cta *c) { c->rng ^= c->rng << 13; c->rng ^= c->rng >> 7; c->rng ^= c->rng << 17; return c->rng; }
+// the warp to run after warp cur reached a switch point (-1: none is runnable)
+static int pick(Cta *c, int cur)
+{
+	const int W = c->n_warps;
+	auto next_after = [&](int skip) { // round robin from cur, skipping warp `skip`
+		for (int d = 1; d <= W; ++d) { const int x = (cur + d) % W; if (x != skip && runnable(c, &c->w[x])) return x; }
+		return -1;
+	};
+	if (c->sched == SCHED_RANDOM) {
+		int cand[64], m = 0;
+		for (int x = 0; x < W; ++x) if (runnable(c, &c->w[x])) cand[m++] = x;
+		return m ? cand[next_rand(c) % m] : -1;
+	}
+	if (c->sched == SCHED_LAGGARD) { const int x = next_after(c->sched_warp); return x >= 0 ? x : runnable(c, &c->w[c->sched_warp]) ? c->sched_warp : -1; }
+	if (c->sched == SCHED_LEADER && runnable(c, &c->w[c->sched_warp])) return c->sched_warp;
+	return next_after(-1);
+}
+[[noreturn]] static void deadlock(Cta *c) { c->deadlock = 1; setcontext(&c->main_ctx); abort(); }
+// when every warp is blocked, all are tried once more; if no sync or barrier completed since the last such round, none can go on
+static int pick_or_retry(Cta *c, int cur)
+{
+	int x = pick(c, cur);
+	if (x >= 0) return x;
+	if (c->sweeps && c->syncs == c->syncs_at_sweep) deadlock(c);
+	++c->sweeps, c->syncs_at_sweep = c->syncs;
+	for (int k = 0; k < c->n_warps; ++k) c->w[k].blocked_at = -1;
+	if ((x = pick(c, cur)) < 0) deadlock(c);
+	return x;
+}
+static void enter(Warp *to) { ++to->run; to->blocked_at = -1; warp = to, lane = to->cur; }
+// leave warp w (the current lane) for warp x; returns when w runs again
+static void switch_to(Cta *c, Warp *w, int x)
+{
+	Warp *to = &c->w[x];
+	const int me = lane;
+	if (to == w) { ++w->run, w->blocked_at = -1; return; }
+	++c->switches;
+	enter(to);
+	swapcontext(&w->ctx[me], &to->ctx[to->cur]);
+	warp = w, lane = me;
+}
+static void release_barrier(Cta *c)
+{
+	c->bar_arrived = 0, ++c->bar_gen, ++c->syncs, ++c->events, c->polls_since_sync = 0;
+	for (int k = 0; k < c->n_warps; ++k)
+		for (int l = 0; l < 32; ++l) if (c->w[k].state[l] == LANE_BAR) c->w[k].state[l] = LANE_RUN;
+}
+void cta_sync_done(Warp *w)
+{
+	Cta *c = w->cta;
+	++c->syncs, c->polls_since_sync = 0;
+	for (int l = 0; l < 32; ++l) if (w->state[l] == LANE_SYNC) w->state[l] = LANE_RUN;
+	switch_to(c, w, pick(c, w->id)); // (w itself is runnable)
+}
+void cta_poll()
+{
+	Warp *w = warp; Cta *c = w->cta;
+	const int me = lane;
+	++c->polls;
+	if (++c->polls_since_sync > c->poll_bound) deadlock(c);
+	w->state[me] = LANE_POLL, w->polled_in[me] = w->run;
+	if (warp_blocked(w)) { w->blocked_at = c->events; switch_to(c, w, pick_or_retry(c, w->id)); }
+	else yield_lane();
+	w->state[me] = LANE_RUN;
+}
+void cta_barrier()
+{
+	Warp *w = warp; Cta *c = w->cta;
+	const long long gen = c->bar_gen;
+	if (++c->bar_arrived == c->live_threads) { release_barrier(c); switch_to(c, w, pick(c, w->id)); return; }
+	w->state[lane] = LANE_BAR;
+	while (c->bar_gen == gen) {
+		if (warp_blocked(w)) { w->blocked_at = c->events; switch_to(c, w, pick_or_retry(c, w->id)); }
+		else yield_lane();
+	}
+}
+void cta_atomic(int kind, const void *addr, unsigned long long old, bool ok)
+{
+	Warp *w = warp; Cta *c = w->cta;
+	// (a failed compare-and-swap changes nothing another warp could be waiting for)
+	if (c->on_atomic ? c->on_atomic(c->user, kind, w->id, addr, old, ok) && ok : ok) ++c->events;
+}
+// the last lane of w has returned (on its own fiber, which is not resumed again)
+static void cta_warp_finished(Warp *w)
+{
+	Cta *c = w->cta;
+	++c->events, c->live_threads -= 32;
+	if (c->bar_arrived > 0 && c->bar_arrived == c->live_threads) release_barrier(c);
+	bool any = false;
+	for (int k = 0; k < c->n_warps; ++k) any |= c->w[k].n_done < 32;
+	if (!any) setcontext(&c->main_ctx);
+	Warp *to = &c->w[pick_or_retry(c, w->id)];
+	enter(to);
+	setcontext(&to->ctx[to->cur]);
+}
+int run_cta(Cta *c, void (*body)(int tid, void *arg), void *arg)
+{
+	const int W = c->n_warps;
+	if (W < 1 || W > 64) return -1;
+	Warp *ws = new Warp[W];
+	c->w = ws;
+	c->events = c->syncs = c->polls = c->polls_since_sync = c->sweeps = c->syncs_at_sweep = c->switches = c->bar_gen = 0;
+	c->bar_arrived = 0, c->live_threads = 32 * W, c->deadlock = 0;
+	const size_t stack_bytes = (size_t)1 << 17;
+	for (int k = 0; k < W; ++k) {
+		Warp &X = ws[k];
+		memset(X.done, 0, sizeof(X.done)); memset(X.state, 0, sizeof(X.state));
+		X.cur = 0, X.arrived = 0, X.gen = 0, X.body = body, X.arg = arg, X.cta = c, X.id = k, X.n_done = 0, X.run = 0, X.blocked_at = -1;
+		for (int l = 0; l < 32; ++l) {
+			X.polled_in[l] = -1;
+			X.stack[l] = (char*)malloc(stack_bytes);
+			getcontext(&X.ctx[l]);
+			X.ctx[l].uc_stack.ss_sp = X.stack[l], X.ctx[l].uc_stack.ss_size = stack_bytes, X.ctx[l].uc_link = 0;
+			makecontext(&X.ctx[l], (void (*)())fiber_entry, 0);
+		}
+	}
+	Warp *saved = warp; const int saved_lane = lane;
+	Warp *first = &ws[pick(c, W - 1)];
+	enter(first);
+	swapcontext(&c->main_ctx, &first->ctx[0]);
+	warp = saved, lane = saved_lane;
+	for (int k = 0; k < W; ++k) { g_total_syncs += ws[k].gen; for (int l = 0; l < 32; ++l) free(ws[k].stack[l]); }
+	delete[] ws;
+	c->w = 0;
+	return c->deadlock ? -1 : 0;
 }
 }
 // defined by the CUDA library (ksw_extd2.cu); not used by the sweep itself
@@ -190,7 +330,7 @@ static void run_ring(const wm128_dev *a, int n, const wm_chain_params *P, int32_
 	wm_chain_fill_warp_ring<RING>(a, n, *P, f, p, t, v, ring, lane);
 }
 // the tile formulation (wm_chain_tile_scan): what one CTA of csrc/chain.cu does, with the 32 anchors of a tile taken in
-// order by one software warp (the order satisfies every dependency; the concurrency itself is exercised on the GPU)
+// order by one software warp (the order satisfies every dependency; the concurrency is exercised by tile_cta_emul.cpp and on the GPU)
 static void run_tile(const wm128_dev *a, int n, const wm_chain_params *P, int32_t *f, int32_t *p, int32_t *t, int32_t *v, int lane)
 {
 	static thread_local wm_chain_tile_sm *S = 0;

@@ -135,13 +135,26 @@ def _span_tandem(rng):
     return ol.oracle_sort128(a)  # ties in x are ordered by y, flags included
 
 
+def _giant_chain_arrays():
+    from test_chain_tile_cta import deep_array, zone_array
+    rng = np.random.default_rng(78)
+    return [_tandem_anchors(rng, 120, 100, 171), _tandem_anchors(rng, 300, 200, 340), _tandem_anchors(rng, 60, 40, 64), make_anchors(rng, 9000, repeats=True),
+            make_anchors(rng, 5000, repeats=False), make_anchors(rng, 33, repeats=True), make_anchors(rng, 1, repeats=False),
+            make_span_anchors(rng, 9000, repeats=True), make_span_anchors(rng, 5000, repeats=False), _span_tandem(rng), deep_array(), zone_array()]
+
+
 @pytest.mark.parametrize("tile_min", [None, 1])
 def test_chain_giant_tasks_match_oracle(tile_min, tmp_path):
     """Giant tasks go through the tile kernel (one CTA per task, one warp per anchor of a 32-anchor tile, csrc/chain.cu): tandem
-    lattices of up to 60 000 anchors and dense repeats, against the oracle.  tile_min = 1 sends every task through that kernel.
-    In a child process: the kernel spins on shared-memory flags, a bug there must not hang the session."""
+    lattices of up to 60 000 anchors, dense repeats and arrays crafted so that scans need the anchors below the kernel's ring (the
+    locked deep path), against the oracle.  tile_min = 1 sends every task through that kernel.  In a child process: the kernel spins
+    on shared-memory flags, a bug there must not hang the session."""
     import subprocess
     import sys
+    from test_chain_tile_cta import tile_kernel_reach
+    # on the CPU at the kernel's constants, before the device runs: deep scans, a tile of them, list refills
+    n_deep, per_tile, n_refill = tile_kernel_reach(_giant_chain_arrays(), [(5000, 1000, 5000, 500, 25, 5000)])
+    assert n_deep > 0 and per_tile >= 8 and n_refill > 0, (n_deep, per_tile, n_refill)
     code = r'''
 import sys
 sys.path.insert(0, %r); sys.path.insert(0, %r)
@@ -149,11 +162,8 @@ import numpy as np
 import oracle_lib as ol
 from winnowmap_b200 import kernels
 from test_oracle_vs_ref import make_anchors, make_span_anchors
-from test_gpu_stages import _tandem_anchors, _span_tandem
-rng = np.random.default_rng(78)
-arrays = [_tandem_anchors(rng, 120, 100, 171), _tandem_anchors(rng, 300, 200, 340), _tandem_anchors(rng, 60, 40, 64), make_anchors(rng, 9000, repeats=True),
-          make_anchors(rng, 5000, repeats=False), make_anchors(rng, 33, repeats=True), make_anchors(rng, 1, repeats=False),
-          make_span_anchors(rng, 9000, repeats=True), make_span_anchors(rng, 5000, repeats=False), _span_tandem(rng)]
+from test_gpu_stages import _giant_chain_arrays
+arrays = _giant_chain_arrays()
 for prm in [dict(max_dist_x=5000, min_dist_x=1000, max_dist_y=5000, bw=500), dict(max_dist_x=16000, min_dist_x=1000, max_dist_y=16000, bw=2000),
             dict(max_dist_x=5000, min_dist_x=50, max_dist_y=5000, bw=500, max_iter=20, max_skip=3)]:
     got = kernels.chain_dp_batch(arrays, **prm)

@@ -17,13 +17,13 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+from test_chain_tile_cta import deep_array, tile_kernel_reach, zone_array
 from test_gpu_stages import _span_tandem, _tandem_anchors
 from test_oracle_vs_ref import FLAGS, make_anchors, make_span_anchors, rand_pair
 
 pytestmark = pytest.mark.gpu
 TESTS_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT_DIR = os.path.dirname(TESTS_DIR)
-WM_CT_RING = 4096  # csrc/chain_dev.cuh: the tile kernel's ring; windows longer than WM_CT_RING - 64 take the locked deep scan
 
 _CHILD = r'''
 import sys
@@ -170,17 +170,6 @@ def test_sort_task_loop_matches_oracle(sort_case, env, tmp_path):
 CHAIN_PRM = [(5000, 1000, 5000, 500, 25, 5000), (16000, 1000, 16000, 2000, 25, 5000), (5000, 50, 5000, 500, 3, 20)]
 
 
-def _window_span(a, mx, mn, it):
-    """max over i of i - st[i], st[i] of src/chain.c:49-55 in closed form: max(lb(max_dist_x), min(i - max_iter, lb(min_dist_x)))
-    with lb(d) the first s whose x + d >= x[i]."""
-    x = a[:, 0]
-    lb = lambda d: np.searchsorted(x, np.where(x > np.uint64(d), x - np.uint64(d), np.uint64(0)), side="left")
-    i = np.arange(len(x))
-    st = lb(mx)
-    st = np.where(i - st > it, np.maximum(st, np.minimum(i - it, lb(mn))), st)
-    return int((i - st).max()) if len(x) else 0
-
-
 @pytest.fixture(scope="module")
 def chain_case(tmp_path_factory, n_sm):
     rng = np.random.default_rng(79)
@@ -188,9 +177,12 @@ def chain_case(tmp_path_factory, n_sm):
              make_span_anchors(rng, 9000, repeats=True), _span_tandem(rng), make_anchors(rng, 5000, repeats=False),
              make_span_anchors(rng, 5000, repeats=False), make_span_anchors(rng, 4097, repeats=True), _tandem_anchors(rng, 80, 50, 200),
              make_anchors(rng, 3000, repeats=True), _tandem_anchors(rng, 60, 40, 64), make_anchors(rng, 2049, repeats=False)]
-    assert len(giant) >= 12 and min(len(a) for a in giant) == 2049
-    # one window spans more anchors than the tile kernel's ring keeps: the locked deep scan runs
-    assert _window_span(giant[0], *CHAIN_PRM[0][:2], CHAIN_PRM[0][5]) > WM_CT_RING - 64
+    giant += [deep_array(), zone_array()]  # candidates below the tile kernel's ring, by construction (test_chain_tile_cta.py)
+    assert len(giant) >= 14 and min(len(a) for a in giant) == 2049
+    # checked on the CPU at the tile kernel's constants before anything runs on the device: scans that need the locked deep path,
+    # whole groups of them in one tile (warps contend for the lock), and scans that refill the candidate list
+    n_deep, per_tile, n_refill = tile_kernel_reach(giant, CHAIN_PRM)
+    assert n_deep > 0 and per_tile >= 8 and n_refill > 0, (n_deep, per_tile, n_refill)
     # medium tasks (129-2048 anchors): more than the ring kernel's warps at any ring size (3 CTAs of 4 warps per SM at 512)
     medium = [(make_span_anchors if j % 3 == 0 else make_anchors)(rng, int(n), repeats=bool(j & 1))
               for j, n in enumerate(rng.integers(129, 2049, size=3 * n_sm * 4 + 40))]

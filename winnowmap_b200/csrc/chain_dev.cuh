@@ -359,7 +359,7 @@ __device__ void wm_chain_fill_warp_ring(const wm128_dev *__restrict__ a, int n, 
 #define WM_LDCG(p) __ldcg(p)
 #endif
 #ifndef WM_CT_RING
-#define WM_CT_RING 4096 // (the CPU emulation harness of the tests builds with a small ring to force the locked deep path)
+#define WM_CT_RING 4096 // (the single-warp emulation of the tests builds with a small ring to force the locked deep path; their CTA emulation keeps this one)
 #endif
 // List capacity per warp.  On tandem lattices with the map-ont options the reference's loop consumes 35 candidates per
 // anchor in the median, 43 at the 99th percentile (tools/bench_chain.py --counts); a longer list would only make phase A
