@@ -67,7 +67,8 @@ int wm_ksw_extd2_batch(int n, const uint8_t *qseq, const int64_t *qoff, const ui
  * calls when MM_F_SPLICE is set (src/align.c:326-327): m = 5, no band, no end bonus.  flag: the KSW_EZ_* bits of
  * src/ksw2.h:7-17, including SPLICE_FOR 0x100 / SPLICE_REV 0x200 / SPLICE_FLANK 0x400.  junc: one annotation byte per
  * target base (mm_idx_bed_junc, src/index.c:780), same offsets as tseq, or NULL.  The kernel is complete and parity-
- * tested; the mapper itself still refuses -x splice (the splice branches of mm_align1 are not built). */
+ * tested; the mapper maps -x splice without base alignment and refuses it with MM_F_CIGAR (the splice branches of
+ * mm_align1 are not built). */
 int wm_ksw_exts2_batch(int n, const uint8_t *qseq, const int64_t *qoff, const uint8_t *tseq, const int64_t *toff, const uint8_t *junc,
                        const int8_t *mat, int q, int e, int q2, int noncan, int junc_bonus,
                        const int32_t *zdrop, const int32_t *flag, wm_extz_t *ez, uint32_t *cigar, const int64_t *cigar_off);
@@ -100,9 +101,15 @@ int wm_sketch_batch_hpc(const wm_bloom_t *bloom, int n, const char *seq, const i
  * array i is a[off[i] .. off[i+1]); sorted in place with the reference's tie order. */
 int wm_radix_sort_128x_batch(int n_arr, wm128_t *a, const int64_t *off);
 
-/* Batched mm_chain_dp (src/chain.c:22; prototype src/mmpriv.h:67) for n_segs = 1,
- * is_cdna = 0.  Anchors of task i: a[off[i] .. off[i+1]) (sorted as by collect_seed_hits).
+/* Batched mm_chain_dp (src/chain.c:22; prototype src/mmpriv.h:67) for n_segs = 1 and is_cdna as given: nonzero
+ * is the gap cost of spliced mapping (src/chain.c:69-77), which the mapper uses under MM_F_SPLICE.
+ * Anchors of task i: a[off[i] .. off[i+1]) (sorted as by collect_seed_hits).
  * Outputs: n_u[i]; u at u[off[i] .. +n_u[i]); chained anchors at b[off[i] .. +n_b[i]). */
+int wm_chain_dp_batch_cdna(int n_tasks, const wm128_t *a, const int64_t *off,
+                           int max_dist_x, int min_dist_x, int max_dist_y, int bw, int max_skip, int max_iter,
+                           int min_cnt, int min_sc, float gap_scale, int is_cdna,
+                           int32_t *n_u, uint64_t *u, wm128_t *b, int64_t *n_b);
+/* The same with is_cdna = 0. */
 int wm_chain_dp_batch(int n_tasks, const wm128_t *a, const int64_t *off,
                       int max_dist_x, int min_dist_x, int max_dist_y, int bw, int max_skip, int max_iter,
                       int min_cnt, int min_sc, float gap_scale,
@@ -220,9 +227,13 @@ typedef struct { /* mm_mapopt_t, src/minimap.h:112-176 */
 
 
 /* mm_set_opt / mm_check_opt (src/options.c:89,133): same presets, same return codes, plus -7 for two gap pairs whose
-   int8 lanes in the reference's ksw_extd2_sse can wrap (-A + q + 2e > 128), which the device fill does not reproduce */
+   int8 lanes in the reference's ksw_extd2_sse can wrap (-A + q + 2e > 128), which the device fill does not reproduce, and
+   -8 for MM_F_SPLICE together with MM_F_CIGAR: spliced mapping (splice, splice:hq, cdna, --splice) is built without its
+   base-level alignment.  mm_mapopt_max_intron_len (src/options.c:83-87, -G): max_gap_ref = bw = max_intron_len when
+   MM_F_SPLICE is set and max_intron_len > 0, else nothing; apply it after the preset, as the CLI does. */
 int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo);
 int wm_check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo);
+void wm_mapopt_max_intron_len(wm_mapopt_t *opt, int max_intron_len);
 int wm_sizeof_mapopt(void);
 int wm_sizeof_reg1(void);
 /* sizeof(wm_mapopt_t / wm_reg1_t / wm_extra_t / wm_idxopt_t) followed by the offset of every addressable field, in
@@ -310,7 +321,8 @@ wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
  * opt->flag may carry MM_F_NO_DIAG (-D), MM_F_NO_DUAL (--dual=no), both with MM_F_ALL_CHAINS | MM_F_NO_LJOIN (-X), and
  * MM_F_FOR_ONLY / MM_F_REV_ONLY (--for-only / --rev-only): the seed filter of skip_seed (src/map.c:132-154) runs on the
  * device.  Its name tests compare names[i] with the index's sequence names; names == NULL or names[i] == NULL is a read
- * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE, MM_F_SR and MM_F_HEAP_SORT are refused. */
+ * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE maps with the cDNA chaining of the reference;
+ * with MM_F_CIGAR it is refused (wm_check_opt's -8), as are MM_F_SR and MM_F_HEAP_SORT. */
 int wm_gpu_map_batch(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, int n_seq, const char *const *names, const char *const *seqs,
                      const int32_t *lens, int32_t *n_reg, wm_reg1_t **reg, int32_t *rep_len, int32_t *frag_gap, int n_threads);
 

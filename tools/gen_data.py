@@ -133,6 +133,97 @@ def make_reads(rng, contigs, n_reads, n50, err, min_len=1000, max_len=200000):
     return recs
 
 
+def _revcomp(seq):
+    return COMP[seq[::-1]]
+
+
+def make_transcriptome(rng, genome_len, n_genes, n_contigs=2, long_introns=2, long_genes=3, n_paralogs=3):
+    """A seeded spliced-transcript setting: (contigs, transcripts).  contigs: i.i.d. genome sequence with multi-exon genes on
+    both strands.  Introns are GT-AG on the plus strand and CT-AC (their reverse complement) on the minus strand, except about
+    one in twenty, which keeps random donor / acceptor bases; their lengths are log-uniform from 60 bp to 20 kb, plus
+    `long_introns` introns above 200 kb.  The first `long_genes` genes have a long last exon, so that their transcripts exceed
+    10 kb.  Every gene of three or more exons also gets an isoform that skips one internal exon, and `n_paralogs` genes get a
+    copy elsewhere (exons 3 % divergent, introns of their own).  transcripts: (name, mRNA as uint8 in the gene's sense, 5' to 3')."""
+    contigs = [random_seq(rng, genome_len // n_contigs) for _ in range(n_contigs)]
+    cursor = [1000] * n_contigs
+    exon_seqs, transcripts, n_long = [], [], 0
+
+    def intron_lengths(ne, g):
+        nonlocal n_long
+        introns = [int(round(math.exp(rng.uniform(math.log(60), math.log(20000))))) for _ in range(ne - 1)]
+        if n_long < long_introns and g >= long_genes and ne > 2:
+            introns[(ne - 1) // 2] = int(rng.integers(200500, 230000))
+            n_long += 1
+        return introns
+
+    def place(name, bodies, introns, strand, ci):
+        seq = contigs[ci]
+        span = sum(len(x) for x in bodies) + sum(introns)
+        start = cursor[ci] + int(rng.integers(2000, 20000))
+        if start + span + 1000 > len(seq):
+            return None
+        cursor[ci] = start + span
+        pos, parts = start, []
+        for e, body in enumerate(bodies):
+            seq[pos:pos + len(body)] = body
+            parts.append(body)
+            pos += len(body)
+            if e < len(introns):
+                end = pos + introns[e]
+                if rng.random() >= 0.05:
+                    seq[pos:pos + 2] = np.frombuffer(b"GT" if strand == "+" else b"CT", np.uint8)
+                    seq[end - 2:end] = np.frombuffer(b"AG" if strand == "+" else b"AC", np.uint8)
+                pos = end
+        isoforms = [parts]
+        if len(parts) >= 3:
+            skip = int(rng.integers(1, len(parts) - 1))
+            isoforms.append(parts[:skip] + parts[skip + 1:])
+        for iso, ps in enumerate(isoforms):
+            m = np.concatenate(ps)
+            transcripts.append((f"{name}.{iso}{strand}", m if strand == "+" else _revcomp(m)))
+        return parts
+
+    for g in range(n_genes):
+        ne = int(rng.integers(2, 11))
+        lens = [int(x) for x in rng.integers(80, 400, ne)]
+        lens[0] += int(rng.integers(50, 300))
+        lens[-1] = int(rng.integers(9000, 13000)) if g < long_genes else lens[-1] + int(rng.integers(200, 1500))
+        parts = place(f"g{g}", [random_seq(rng, L) for L in lens], intron_lengths(ne, g), "+" if rng.random() < 0.5 else "-", g % n_contigs)
+        if parts is not None:
+            exon_seqs.append(parts)
+    for p in range(min(n_paralogs, len(exon_seqs))):
+        src = exon_seqs[int(rng.integers(0, len(exon_seqs)))]
+        bodies = [mutate(rng, x, 0.03, split=(1.0, 0.0, 0.0)) for x in src]
+        place(f"p{p}", bodies, intron_lengths(len(bodies), long_genes), "+" if rng.random() < 0.5 else "-", p % n_contigs)
+    return [(f"chr{i + 1}", c) for i, c in enumerate(contigs)], transcripts
+
+
+def make_spliced_reads(rng, contigs, transcripts, n_reads, err, n_genomic=0, n_random=0, min_len=200):
+    """cDNA-like reads of `transcripts` (make_transcriptome): full length or 5'-truncated, a poly(A) tail of 10-40 bases, either
+    orientation, ONT-like i.i.d. errors at rate err; plus n_genomic unspliced genomic reads (1-5 kb) and n_random random ones."""
+    recs = []
+    for i in range(n_reads):
+        name, m = transcripts[int(rng.integers(0, len(transcripts)))]
+        if rng.random() < 0.5 and len(m) > 2 * min_len:
+            m = m[int(rng.integers(0, len(m) - min_len)):]
+        m = np.concatenate([m, np.full(int(rng.integers(10, 41)), ord("A"), np.uint8)])
+        strand = "+"
+        if rng.random() < 0.5:
+            m, strand = _revcomp(m), "-"
+        recs.append((f"t{i}_{name}_{strand}", mutate(rng, m, err)))
+    for i in range(n_genomic):
+        ci = int(rng.integers(0, len(contigs)))
+        L = int(rng.integers(1000, 5001))
+        st = int(rng.integers(0, len(contigs[ci][1]) - L))
+        frag = contigs[ci][1][st:st + L]
+        if rng.random() < 0.5:
+            frag = _revcomp(frag)
+        recs.append((f"gen{i}_{contigs[ci][0]}_{st}", mutate(rng, frag, err)))
+    for i in range(n_random):
+        recs.append((f"rand{i}", random_seq(rng, int(rng.integers(300, 3000)))))
+    return recs
+
+
 def count_kmers(contigs, k):
     """Canonical k-mer -> count, vectorised (k <= 31)."""
     mask = (1 << (2 * k)) - 1

@@ -674,8 +674,67 @@ def record_occ(tmp):
     return rec
 
 
+# ---- spliced mapping without base alignment (-x splice / splice:hq / cdna, --splice, -G): tests/golden/splice_manifest.json and
+# splice_*; the other manifests are not touched.  Inputs: a transcriptome of gen_data.make_transcriptome (genes on both strands,
+# GT-AG / CT-AC introns from 60 bp to over 200 kb, isoforms, paralogs) and cDNA-like reads of it: "tx" ONT-like, "tx_hq" low
+# error, "tx_long" only transcripts of 10 kb or more (--splice on map-ont: stage 1 runs, with cDNA chaining).
+SPLICE = dict(genome_len=1600000, n_genes=40, ref_seed=1051, read_seed=2051, n_reads=160, n_genomic=16, n_random=4, k=15)
+SPLICE_READS = {"tx": dict(err=0.06, long=False), "tx_hq": dict(err=0.01, long=False), "tx_long": dict(err=0.05, long=True)}
+SPLICE_CASES = {
+    # name: (reads, reference options, -W, library options of Mapper)
+    "splice_W": ("tx", ["-x", "splice"], True, dict(preset="splice", cigar=False)),
+    "splice_noW": ("tx", ["-x", "splice"], False, dict(preset="splice", cigar=False)),
+    "splice_hq": ("tx_hq", ["-x", "splice:hq"], True, dict(preset="splice:hq", cigar=False)),
+    "splice_G20k": ("tx", ["-x", "splice", "-G", "20000"], True, dict(preset="splice", cigar=False, max_intron_len=20000)),
+    "splice_ont_long": ("tx_long", ["-x", "map-ont", "--splice"], True, dict(preset="map-ont", cigar=False, splice=True)),
+    "splice_H": ("tx", ["-x", "splice", "-H"], True, dict(preset="splice", cigar=False, hpc=True)),
+    "splice_I_split": ("tx", ["-x", "splice", "-I", "500k", "--split-prefix", "SPLIT"], True,
+                       dict(preset="splice", cigar=False, part_bases=500000, split=True)),
+}
+
+
+def make_splice_inputs(reads_kind, outdir):
+    """(genome FASTA, reads FASTA, -W file) of one spliced read set."""
+    c, r = SPLICE, SPLICE_READS[reads_kind]
+    os.makedirs(outdir, exist_ok=True)
+    ref, reads, wfile = (os.path.join(outdir, "splice" + x) for x in (".ref.fa", "_" + reads_kind + ".reads.fa", ".rep.txt"))
+    contigs, tx = gen_data.make_transcriptome(np.random.default_rng(c["ref_seed"]), c["genome_len"], c["n_genes"])
+    gen_data.write_fasta(ref, contigs)
+    if r["long"]:
+        tx = [t for t in tx if len(t[1]) >= 10000]
+    rng = np.random.default_rng(c["read_seed"] + len(reads_kind))
+    n = c["n_reads"] // 4 if r["long"] else c["n_reads"]
+    recs = gen_data.make_spliced_reads(rng, contigs, tx, n, r["err"], 0 if r["long"] else c["n_genomic"], 0 if r["long"] else c["n_random"])
+    gen_data.write_fasta(reads, recs)
+    gen_data.write_top_kmers(wfile, contigs, c["k"], 0.9998)
+    return ref, reads, wfile
+
+
+def main_splice():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_splice"
+    manifest = {}
+    for name, (reads_kind, args, use_w, lib_opts) in SPLICE_CASES.items():
+        ref, reads, wfile = make_splice_inputs(reads_kind, tmp)
+        args = [a if a != "SPLIT" else os.path.join(tmp, name + ".split") for a in args]
+        cmd = [refbin, "-t", "4"] + args + (["-W", wfile] if use_w else []) + [ref, reads]
+        out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+        with gzip.GzipFile(os.path.join(gdir, name + ".paf.gz"), "wb", mtime=0) as f:
+            f.write(out)
+        manifest[name] = dict(reads=reads_kind, use_W=use_w, lib=lib_opts, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile) if use_w else None,
+                              cmd=" ".join(["winnowmap"] + [a if not a.startswith(tmp) else "<prefix>" for a in cmd[1:-2]] + ["ref.fa", "reads.fa"]),
+                              paf_md5=hashlib.md5(out).hexdigest(), n_lines=out.count(b"\n"))
+        print(name, manifest[name]["n_lines"], "lines")
+    json.dump(manifest, open(os.path.join(gdir, "splice_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
-    if "--hpc" in sys.argv:
+    if "--splice" in sys.argv:
+        main_splice()
+    elif "--hpc" in sys.argv:
         main_hpc()
     elif "--overlap" in sys.argv:
         main_overlap()

@@ -50,5 +50,6 @@ def lib():
         L.wm_sketch_batch_hpc.argtypes = L.wm_sketch_batch.argtypes
         L.wm_radix_sort_128x_batch.argtypes = [C.c_int, u64p, i64p]
         L.wm_chain_dp_batch.argtypes = [C.c_int, u64p, i64p] + [C.c_int] * 8 + [C.c_float, i32p, u64p, u64p, i64p]
+        L.wm_chain_dp_batch_cdna.argtypes = [C.c_int, u64p, i64p] + [C.c_int] * 8 + [C.c_float, C.c_int, i32p, u64p, u64p, i64p]
         _lib = L
     return _lib

@@ -474,6 +474,7 @@ extern "C" int64_t wm_topfreq(const char *ref_fn, int k, double distinct, uint64
 
 extern "C" int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo) { return set_opt(preset, io, mo); }
 extern "C" int wm_check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo) { return check_opt(io, mo); }
+extern "C" void wm_mapopt_max_intron_len(wm_mapopt_t *opt, int max_intron_len) { mapopt_max_intron_len(opt, max_intron_len); }
 // mm_idx_cal_max_occ (src/index.c:173-194) of one index: INT32_MAX for f <= 0, else the ((1 - f) * n)-th smallest occurrence
 // count over the n keys, plus one, selected on the device (occ_select.cu) and remembered per f.  -1, with a message, where
 // the reference would read past its array (the rank reaches n: f too small for the number of keys, or no key at all) and

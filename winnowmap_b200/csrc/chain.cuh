@@ -8,7 +8,10 @@ struct wm_chain_params {
 	float gap_scale;
 };
 
-struct wm_chain_params2 { wm_chain_params p[2]; }; // stage-1/fallback and stage-2 parameter sets
+struct wm_chain_sets { wm_chain_params p[2]; }; // stage-1/fallback and stage-2 parameter sets: what the kernels read
+// is_cdna: the cDNA gap cost of mm_chain_dp (src/chain.c:69-77), the same for both sets (map.c passes is_splice at every call);
+// wm_chain_run launches the instantiation of the forward pass it selects
+struct wm_chain_params2 : wm_chain_sets { int32_t is_cdna = 0; };
 
 struct wm_chain_ws {
 	wm_dbuf f, p, t, v, u, u2, w, b, n_u, n_b, counter, order, stacks;

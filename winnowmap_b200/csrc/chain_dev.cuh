@@ -17,7 +17,9 @@ __device__ __forceinline__ int wm_warp_incl_max(int v, int lane)
 	return v;
 }
 
-// score of predecessor j for anchor i (src/chain.c:61-84); false when j is not a candidate
+// score of predecessor j for anchor i (src/chain.c:61-84); false when j is not a candidate.  CDNA: the gap cost of is_cdna
+// (src/chain.c:69-77 with n_segs == 1): a gap longer on the reference than on the query (an intron) costs min(c_lin, c_log)
+template <bool CDNA = false>
 __device__ __forceinline__ bool wm_chain_score(const wm128_dev aj, uint64_t ri, int32_t qi, int32_t q_span, const wm_chain_params &P, double avg_d, double scale_d, int *sc_out)
 {
 	const int64_t dr = (int64_t)(ri - aj.x);
@@ -29,7 +31,8 @@ __device__ __forceinline__ bool wm_chain_score(const wm128_dev aj, uint64_t ri, 
 	const int32_t min_d = dq < dr ? dq : (int32_t)dr;
 	int sc = min_d > q_span ? q_span : min_d;
 	const int log_dd = dd ? 31 - __clz(dd) : 0;
-	const int gap_cost = (int)__dmul_rn(__dmul_rn((double)dd, .01), avg_d) + (log_dd >> 1);
+	const int c_lin = (int)__dmul_rn(__dmul_rn((double)dd, .01), avg_d);
+	const int gap_cost = CDNA && dr > dq ? (c_lin < log_dd ? c_lin : log_dd) : c_lin + (log_dd >> 1);
 	sc -= (int)__dadd_rn(__dmul_rn((double)gap_cost, scale_d), .499);
 	*sc_out = sc;
 	return true;
@@ -57,6 +60,7 @@ __device__ __forceinline__ int wm_chain_replay(unsigned R, unsigned K, int *n_sk
 }
 
 // one warp, one task
+template <bool CDNA = false>
 __device__ void wm_chain_fill_warp(const wm128_dev *__restrict__ a, int n, const wm_chain_params &P, int32_t *f, int32_t *p, int32_t *t, int32_t *v, int lane)
 {
 	const unsigned FULL = 0xffffffffu;
@@ -79,7 +83,7 @@ __device__ void wm_chain_fill_warp(const wm128_dev *__restrict__ a, int n, const
 			const int j = jb - lane;
 			bool cand = false;
 			int sc = INT_MIN, pj = -1;
-			if (j >= st && wm_chain_score(a[j], ri, qi, q_span, P, avg_d, scale_d, &sc)) {
+			if (j >= st && wm_chain_score<CDNA>(a[j], ri, qi, q_span, P, avg_d, scale_d, &sc)) {
 				sc += f[j]; pj = p[j]; cand = true;
 			}
 			if (cand && pj >= 0) t[pj] = i; // src/chain.c:87 (only indices below every j still to be visited)
@@ -131,6 +135,7 @@ __device__ __forceinline__ bool wm_chain_is_cand(const wm128_dev aj, uint64_t ri
 }
 
 // D: the warp's candidate list (WM_CHAIN_DENSE_CAP entries, shared memory)
+template <bool CDNA = false>
 __device__ void wm_chain_fill_warp_dense(const wm128_dev *__restrict__ a, int n, const wm_chain_params &P, int32_t *f, int32_t *p, int32_t *t, int32_t *v,
                                          int32_t *D, int lane)
 {
@@ -170,7 +175,7 @@ __device__ void wm_chain_fill_warp_dense(const wm128_dev *__restrict__ a, int n,
 			int j = -1, sc = INT_MIN, pj = -1;
 			if (cand) {
 				j = D[lane];
-				wm_chain_score(a[j], ri, qi, q_span, P, avg_d, scale_d, &sc);
+				wm_chain_score<CDNA>(a[j], ri, qi, q_span, P, avg_d, scale_d, &sc);
 				sc += f[j]; pj = p[j];
 			}
 			if (cand && pj >= 0) t[pj] = i;
@@ -245,7 +250,7 @@ template <int RING> struct wm_chain_ring {
 };
 
 // One warp, one task.  v[] holds st[] on entry (wm_chain_window_start of every anchor) and the peak scores on return.
-template <int RING>
+template <int RING, bool CDNA = false>
 __device__ void wm_chain_fill_warp_ring(const wm128_dev *__restrict__ a, int n, const wm_chain_params &P, int32_t *f, int32_t *p, int32_t *t, int32_t *v,
                                         wm_chain_ring<RING> *R, int lane)
 {
@@ -282,7 +287,7 @@ __device__ void wm_chain_fill_warp_ring(const wm128_dev *__restrict__ a, int n, 
 						if (j >= ring_lo) { const int s = j & MASK; aj.x = R->x[s]; aj.y = (uint64_t)(uint32_t)R->q[s]; fj = R->f[s]; pj = R->p[s]; }
 						else { aj = a[j]; fj = f[j]; pj = p[j]; }
 						int s0;
-						if (wm_chain_score(aj, ri, qi, q_span, P, avg_d, scale_d, &s0)) {
+						if (wm_chain_score<CDNA>(aj, ri, qi, q_span, P, avg_d, scale_d, &s0)) {
 							cand[h] = true; sc[h] = s0 + fj;
 							if (pj >= 0) { if (pj >= ring_lo) R->t[pj & MASK] = i; else t[pj] = i; } // src/chain.c:87
 						}
@@ -435,13 +440,14 @@ __device__ __forceinline__ wm128_dev wm_chain_coords(const wm128_dev *__restrict
 
 // Phase A from predecessor jtop down: lane m looks at j = jtop - m, 32 per step, until the list is full or the window is
 // exhausted.  Returns the next predecessor to look at (< st: the window is exhausted).
+template <bool CDNA = false>
 __device__ __forceinline__ int wm_chain_list_fill(const wm128_dev *__restrict__ a, const wm_chain_tile_sm *S, const wm_chain_scan &A, const wm_chain_params &P,
                                                   int2 *L, int *cnt, int cap, int jtop, int st, int i0, int ring_lo, double avg_d, double scale_d, int lane)
 {
 	while (jtop >= st && *cnt < cap) {
 		const int j = jtop - lane;
 		int s0 = 0;
-		const bool c = j >= st && wm_chain_score(wm_chain_coords(a, S, j, i0, ring_lo), A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
+		const bool c = j >= st && wm_chain_score<CDNA>(wm_chain_coords(a, S, j, i0, ring_lo), A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
 		const unsigned m = __ballot_sync(0xffffffffu, c);
 		const int jr = wm_chain_list_append(L, cnt, cap, c, j, s0, m, __popc(m & ((1u << lane) - 1u)));
 		if (jr != INT_MIN) return jr;
@@ -454,6 +460,7 @@ __device__ __forceinline__ int wm_chain_list_fill(const wm128_dev *__restrict__ 
 // two steps cover the two register tiles, tile aligned (lane l looks at i0 + l, then at i0 - 32 + l; scan order is descending
 // lane order): *Cc / *Cp receive the candidates among them, which are what anchor i has to wait for.  Returns the next predecessor
 // to look at; *cnt receives the length of the list.
+template <bool CDNA = false>
 __device__ __forceinline__ int wm_chain_list_begin(const wm128_dev *__restrict__ a, const wm_chain_tile_sm *S, const wm_chain_scan &A, const wm_chain_params &P,
                                                    int2 *L, int cap, wm128_dev cur, wm128_dev prev, int i0, int k, int st, int ring_lo, double avg_d, double scale_d,
                                                    int lane, int *cnt, unsigned *Cc, unsigned *Cp)
@@ -464,7 +471,7 @@ __device__ __forceinline__ int wm_chain_list_begin(const wm128_dev *__restrict__
 	{
 		const int j = i0 + lane;
 		int s0 = 0;
-		const bool c = lane < k && j >= st && wm_chain_score(cur, A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
+		const bool c = lane < k && j >= st && wm_chain_score<CDNA>(cur, A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
 		const unsigned m = __ballot_sync(FULL, c);
 		*Cc = m;
 		jr = wm_chain_list_append(L, cnt, cap, c, j, s0, m, __popc(m >> lane >> 1));
@@ -472,19 +479,20 @@ __device__ __forceinline__ int wm_chain_list_begin(const wm128_dev *__restrict__
 	{
 		const int j = i0 - 32 + lane;
 		int s0 = 0;
-		const bool c = j >= st && wm_chain_score(prev, A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
+		const bool c = j >= st && wm_chain_score<CDNA>(prev, A.ri, A.qi, A.q_span, P, avg_d, scale_d, &s0);
 		const unsigned m = __ballot_sync(FULL, c);
 		*Cp = m;
 		if (jr == INT_MIN) jr = wm_chain_list_append(L, cnt, cap, c, j, s0, m, __popc(m >> lane >> 1));
 	}
 	if (jr != INT_MIN) return jr;
-	return wm_chain_list_fill(a, S, A, P, L, cnt, cap, i0 - 33, st, i0, ring_lo, avg_d, scale_d, lane);
+	return wm_chain_list_fill<CDNA>(a, S, A, P, L, cnt, cap, i0 - 33, st, i0, ring_lo, avg_d, scale_d, lane);
 }
 
 // Phase B of the scan of anchor A.i: the list (cnt entries, next predecessor jr) was made by wm_chain_list_begin, and every
 // listed entry at or above ring_lo has published.  f / p of entries j >= ring_lo come from the ring; older ones from global
 // memory, and only when deep_ok (the caller holds the lock: the global t[] marks are then this anchor's alone).  Returns false
 // if it would have had to go below the ring without deep_ok; on success A.max_f / A.max_j hold f[i] / p[i].
+template <bool CDNA = false>
 __device__ __forceinline__ bool wm_chain_list_resolve(const wm128_dev *__restrict__ a, const wm_chain_params &P, const int32_t *f, const int32_t *p, int32_t *t,
                                                       wm_chain_tile_sm *S, uint32_t *mk, int2 *L, int cap, wm_chain_scan &A, int cnt, int jr, int st, int i0,
                                                       int ring_lo, bool deep_ok, double avg_d, double scale_d, int lane)
@@ -524,7 +532,7 @@ __device__ __forceinline__ bool wm_chain_list_resolve(const wm128_dev *__restric
 		// of anchor i has published by now)
 		__syncwarp();
 		cnt = 0;
-		jr = wm_chain_list_fill(a, S, A, P, L, &cnt, cap, jr, st, i0, ring_lo, avg_d, scale_d, lane);
+		jr = wm_chain_list_fill<CDNA>(a, S, A, P, L, &cnt, cap, jr, st, i0, ring_lo, avg_d, scale_d, lane);
 		__syncwarp();
 	}
 }
@@ -534,7 +542,7 @@ struct wm_chain_no_wait { __device__ void operator()(unsigned, unsigned) const {
 // The scan of anchor i = i0 + k by warp k: phase A into the warp's list S->list[k] (at most cap entries), then wait(Cc, Cp) with the
 // candidates of the two register tiles (cur / prev: lane l holds a[i0 + l] / a[i0 - 32 + l]), then phase B.  Returns false if it
 // would have had to go below the ring without deep_ok; on success *mf / *mj hold f[i] / p[i].
-template <class Wait = wm_chain_no_wait>
+template <bool CDNA = false, class Wait = wm_chain_no_wait>
 __device__ __forceinline__ bool wm_chain_tile_scan(const wm128_dev *__restrict__ a, const wm_chain_params &P, const int32_t *f, const int32_t *p, int32_t *t,
                                                    wm_chain_tile_sm *S, uint32_t *mk, wm128_dev cur, wm128_dev prev, int i0, int k, int st, int ring_lo, bool deep_ok,
                                                    double avg_d, double scale_d, int lane, int *mf, int *mj, Wait wait = Wait(), int cap = WM_CT_LIST)
@@ -545,9 +553,9 @@ __device__ __forceinline__ bool wm_chain_tile_scan(const wm128_dev *__restrict__
 	{ const uint64_t yi = __shfl_sync(FULL, cur.y, k); A.qi = (int32_t)yi, A.q_span = (int32_t)(yi >> 32 & 0xff); }
 	int2 *L = S->list[k];
 	int cnt; unsigned Cc, Cp;
-	const int jr = wm_chain_list_begin(a, S, A, P, L, cap, cur, prev, i0, k, st, ring_lo, avg_d, scale_d, lane, &cnt, &Cc, &Cp);
+	const int jr = wm_chain_list_begin<CDNA>(a, S, A, P, L, cap, cur, prev, i0, k, st, ring_lo, avg_d, scale_d, lane, &cnt, &Cc, &Cp);
 	wait(Cc, Cp);
-	if (!wm_chain_list_resolve(a, P, f, p, t, S, mk, L, cap, A, cnt, jr, st, i0, ring_lo, deep_ok, avg_d, scale_d, lane)) return false;
+	if (!wm_chain_list_resolve<CDNA>(a, P, f, p, t, S, mk, L, cap, A, cnt, jr, st, i0, ring_lo, deep_ok, avg_d, scale_d, lane)) return false;
 	*mf = A.max_f, *mj = A.max_j;
 	return true;
 }

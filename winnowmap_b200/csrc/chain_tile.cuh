@@ -5,9 +5,10 @@
 // WM_CT_WARPS * 32.  S: the dynamic shared memory, s_task / s_sum: the kernel's static shared variables.  A function of its own so that
 // the tests can run it, unchanged, on an emulated CTA (tests/hostsim/tile_cta_emul.cpp).  It lives apart from chain_dev.cuh, whose
 // warp-level functions also compile for the host with nothing but the warp intrinsics: this one needs the CTA ones (__syncthreads,
-// __nanosleep, atomicCAS, atomicExch, __threadfence_block, __ldcg).
+// __nanosleep, atomicCAS, atomicExch, __threadfence_block, __ldcg).  CDNA: the gap cost of is_cdna (wm_chain_score).
+template <bool CDNA = false>
 __device__ __forceinline__ void wm_chain_fill_tile_cta(const wm128_dev *__restrict__ a_all, const int64_t *__restrict__ off, const int32_t *__restrict__ order, int first,
-                                                       int last, const wm_chain_params2 &PP, const uint8_t *__restrict__ set_id, int32_t *__restrict__ f_all,
+                                                       int last, const wm_chain_sets &PP, const uint8_t *__restrict__ set_id, int32_t *__restrict__ f_all,
                                                        int32_t *__restrict__ p_all, int32_t *__restrict__ t_all, int32_t *__restrict__ v_all, int *counter,
                                                        wm_chain_tile_sm *S, int *s_task, unsigned long long *s_sum, int tid)
 {
@@ -63,11 +64,11 @@ __device__ __forceinline__ void wm_chain_fill_tile_cta(const wm128_dev *__restri
 					__threadfence_block();
 				};
 				int max_f, max_j;
-				if (!wm_chain_tile_scan(a, P, f, p, t, S, mk, cur, prev, i0, k, st, ring_lo, false, avg_d, scale_d, lane, &max_f, &max_j, wait)) {
+				if (!wm_chain_tile_scan<CDNA>(a, P, f, p, t, S, mk, cur, prev, i0, k, st, ring_lo, false, avg_d, scale_d, lane, &max_f, &max_j, wait)) {
 					if (lane == 0) { while (atomicCAS(&S->lock, 0, 1) != 0) __nanosleep(64); }
 					__syncwarp();
 					__threadfence_block();
-					wm_chain_tile_scan(a, P, f, p, t, S, mk, cur, prev, i0, k, st, ring_lo, true, avg_d, scale_d, lane, &max_f, &max_j);
+					wm_chain_tile_scan<CDNA>(a, P, f, p, t, S, mk, cur, prev, i0, k, st, ring_lo, true, avg_d, scale_d, lane, &max_f, &max_j);
 					__syncwarp();
 					__threadfence_block();
 					if (lane == 0) atomicExch(&S->lock, 0);

@@ -360,6 +360,7 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 		P.max_dist_x = cp[s].max_dist_x, P.min_dist_x = cp[s].min_dist_x, P.max_dist_y = cp[s].max_dist_y, P.bw = cp[s].bw;
 		P.max_skip = cp[s].max_skip, P.max_iter = cp[s].max_iter, P.min_cnt = cp[s].min_cnt, P.min_sc = cp[s].min_sc, P.gap_scale = cp[s].gap_scale;
 	}
+	PP.is_cdna = cp[0].is_cdna;
 	double t_chain0 = Timers::now();
 	wm_chain_run(&g.ch, d_A, d_foff, f_off.data(), n, PP, d_set, st);
 	g.h_nu.assign(n, 0); g.h_nb.assign(n, 0);

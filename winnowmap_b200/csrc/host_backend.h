@@ -41,6 +41,7 @@ uint32_t skip_bits(const wm_host_idx *mi, int64_t flag, const wm_read *rd, uint3
 struct ChainParams { // arguments of mm_chain_dp (src/chain.c:22)
 	int32_t max_dist_x, min_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc;
 	float gap_scale;
+	int32_t is_cdna = 0; // MM_F_SPLICE of the user's options, in both stages (src/map.c:282)
 };
 
 struct SeedOut { // views into backend-owned host buffers, valid until the next seed_chain call

@@ -62,7 +62,7 @@ void mapopt_init(wm_mapopt_t *o)
 }
 
 int set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo)
-{ // mm_set_opt :89-131 (presets of the accelerated path; splice presets are refused by the mapper)
+{ // mm_set_opt :89-131 (the splice presets map without base alignment: check_opt refuses them with MM_F_CIGAR)
 	if (preset == 0) { idxopt_init(io); mapopt_init(mo); }
 	else if (strcmp(preset, "map-ont") == 0) { io->flag = 0, io->k = 15; }
 	else if (strcmp(preset, "map-pb") == 0) {
@@ -84,8 +84,24 @@ int set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo)
 		io->flag = 0, io->k = 19;
 		mo->a = 1, mo->b = 4, mo->q = 6, mo->q2 = 26, mo->e = 2, mo->e2 = 1, mo->zdrop = mo->zdrop_inv = 200;
 		mo->min_dp_max = 200;
+	} else if (strncmp(preset, "splice", 6) == 0 || strcmp(preset, "cdna") == 0) { // "splice:<anything>" is "splice"
+		mo->SVaware = false;
+		io->w = 25;
+		io->flag = 0, io->k = 15;
+		mo->flag |= WM_F_SPLICE | WM_F_SPLICE_FOR | WM_F_SPLICE_REV | WM_F_SPLICE_FLANK;
+		mo->max_gap = 2000, mo->max_gap_ref = mo->bw = 200000;
+		mo->a = 1, mo->b = 2, mo->q = 2, mo->e = 1, mo->q2 = 32, mo->e2 = 0;
+		mo->noncan = 9;
+		mo->junc_bonus = 9;
+		mo->zdrop = 200, mo->zdrop_inv = 100;
+		if (strcmp(preset, "splice:hq") == 0) mo->junc_bonus = 5, mo->b = 4, mo->q = 6, mo->q2 = 24;
 	} else return -1;
 	return 0;
+}
+
+void mapopt_max_intron_len(wm_mapopt_t *opt, int max_intron_len)
+{ // mm_mapopt_max_intron_len :83-87 (-G): only once MM_F_SPLICE is set
+	if ((opt->flag & WM_F_SPLICE) && max_intron_len > 0) opt->max_gap_ref = opt->bw = max_intron_len;
 }
 
 int check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo)
@@ -106,6 +122,9 @@ int check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo)
 	if ((mo->q != mo->q2 || mo->e != mo->e2) && mo->a + mo->q + 2 * mo->e > 128) return -7;
 	if (mo->zdrop < mo->zdrop_inv) return -5;
 	if ((mo->flag & WM_F_NO_PRINT_2ND) && (mo->flag & WM_F_ALL_CHAINS)) return -5;
+	// Not in the reference either: spliced mapping is built without its base-level alignment (the two-strand ksw_exts2 rounds of
+	// mm_align1 and ts:A), so splice with -c / -a is refused before any mapping instead of printing alignments that differ.
+	if ((mo->flag & WM_F_SPLICE) && (mo->flag & WM_F_CIGAR)) return -8;
 	return 0;
 }
 

@@ -12,6 +12,7 @@ void idxopt_init(wm_idxopt_t *o);
 void mapopt_init(wm_mapopt_t *o);
 int set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo);
 int check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo);
+void mapopt_max_intron_len(wm_mapopt_t *opt, int max_intron_len);
 
 class SeqReader { // FASTA/FASTQ, plain or gzip (kseq semantics, src/kseq.h)
 public:

@@ -89,6 +89,7 @@ ChainParams chain_params(const wm_mapopt_t *o, const wm_mapopt_t *base, int qlen
 	c.max_dist_x = mr, c.min_dist_x = mn, c.max_dist_y = mq, c.bw = o->bw;
 	c.max_skip = o->max_chain_skip, c.max_iter = o->max_chain_iter, c.min_cnt = o->min_cnt, c.min_sc = o->min_chain_score;
 	c.gap_scale = base->chain_gap_scale;
+	c.is_cdna = (base->flag & WM_F_SPLICE) != 0;
 	return c;
 }
 
@@ -135,8 +136,12 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	frag_gap_out.assign(n_reads, 0);
 	if (n_reads == 0) return;
 	if (n_threads < 1) n_threads = 1;
-	if (opt->flag & (WM_F_SPLICE | WM_F_SR | WM_F_HEAP_SORT)) {
-		fprintf(stderr, "[ERROR] winnowmap-b200: splice/sr/heap-sort modes are outside the accelerated path\n");
+	if (opt->flag & (WM_F_SR | WM_F_HEAP_SORT)) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: sr/heap-sort modes are outside the accelerated path\n");
+		exit(1);
+	}
+	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR)) { // check_opt's -8: spliced mapping is built without base alignment
+		fprintf(stderr, "[ERROR] winnowmap-b200: spliced base-level alignment (splice with -c / -a) is not built; map without CIGAR\n");
 		exit(1);
 	}
 	// options the reference honours on this path that are not implemented here are refused, not silently ignored

@@ -155,8 +155,10 @@ def radix_sort_128x_batch(arrays):
     return [flat[off[i]: off[i + 1]].copy() for i in range(n)]
 
 
-def chain_dp_batch(arrays, max_dist_x, min_dist_x, max_dist_y, bw, max_skip=25, max_iter=5000, min_cnt=3, min_sc=40, gap_scale=1.0):
-    """Batched mm_chain_dp (reference src/chain.c:22).  Returns list of (u, b)."""
+def chain_dp_batch(arrays, max_dist_x, min_dist_x, max_dist_y, bw, max_skip=25, max_iter=5000, min_cnt=3, min_sc=40, gap_scale=1.0,
+                   is_cdna=False):
+    """Batched mm_chain_dp (reference src/chain.c:22).  is_cdna=True is the gap cost of spliced mapping (src/chain.c:69-77).
+    Returns list of (u, b)."""
     n = len(arrays)
     off = np.zeros(n + 1, dtype=np.int64)
     if n:
@@ -167,6 +169,10 @@ def chain_dp_batch(arrays, max_dist_x, min_dist_x, max_dist_y, bw, max_skip=25, 
     n_b = np.zeros(max(n, 1), dtype=np.int64)
     u = np.zeros(max(tot, 1), dtype=np.uint64)
     b = np.zeros((max(tot, 1), 2), dtype=np.uint64)
-    lib().wm_chain_dp_batch(n, _p(flat, u64p), _p(off, i64p), max_dist_x, min_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc,
-                            C.c_float(gap_scale), _p(n_u, i32p), _p(u, u64p), _p(b, u64p), _p(n_b, i64p))
+    if is_cdna:
+        lib().wm_chain_dp_batch_cdna(n, _p(flat, u64p), _p(off, i64p), max_dist_x, min_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt,
+                                     min_sc, C.c_float(gap_scale), 1, _p(n_u, i32p), _p(u, u64p), _p(b, u64p), _p(n_b, i64p))
+    else:
+        lib().wm_chain_dp_batch(n, _p(flat, u64p), _p(off, i64p), max_dist_x, min_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc,
+                                C.c_float(gap_scale), _p(n_u, i32p), _p(u, u64p), _p(b, u64p), _p(n_b, i64p))
     return [(u[off[i]: off[i] + n_u[i]].copy(), b[off[i]: off[i] + n_b[i]].copy()) for i in range(n)]

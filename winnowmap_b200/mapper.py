@@ -30,6 +30,7 @@ class MapOpt(C.Structure):  # wm_mapopt_t == mm_mapopt_t (reference src/minimap.
 
 F_CIGAR, F_OUT_SAM, F_OUT_CG, F_NO_PRINT_2ND, F_PAF_NO_HIT = 0x004, 0x008, 0x020, 0x4000, 0x8000000
 F_NO_DIAG, F_NO_DUAL, F_NO_LJOIN, F_FOR_ONLY, F_REV_ONLY, F_ALL_CHAINS = 0x001, 0x002, 0x400, 0x100000, 0x200000, 0x800000
+F_SPLICE, F_SPLICE_FOR, F_SPLICE_REV, F_SPLICE_FLANK = 0x080, 0x100, 0x200, 0x40000
 I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
 
 STAT_NAMES = ("n_reads", "n_bases", "n_minimaps", "n_chained", "n_dp_jobs", "n_ll_jobs", "n_rounds", "t_seed", "t_dp", "t_host",
@@ -41,6 +42,8 @@ def _setup(L):
         return L
     L.wm_set_opt.argtypes = [C.c_char_p, C.POINTER(IdxOpt), C.POINTER(MapOpt)]
     L.wm_check_opt.argtypes = [C.POINTER(IdxOpt), C.POINTER(MapOpt)]
+    L.wm_mapopt_max_intron_len.restype = None
+    L.wm_mapopt_max_intron_len.argtypes = [C.POINTER(MapOpt), C.c_int]
     L.wm_index_build.restype = C.c_void_p
     L.wm_index_build.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_int]
     L.wm_index_build_opt.restype = C.c_void_p
@@ -78,15 +81,26 @@ def _setup(L):
 F_OUT_SAM = 0x008
 
 
-def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, all_vs_all=False, strand=None):
+def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, all_vs_all=False, strand=None, splice=False,
+                 max_intron_len=None):
     """mm_set_opt(0) then mm_set_opt(preset) (reference main.c:144-159); -c sets MM_F_OUT_CG|MM_F_CIGAR, -a sets
     MM_F_OUT_SAM|MM_F_CIGAR (main.c).  Self and all-vs-all mapping: no_diag is -D, dual=False is --dual=no, all_vs_all
-    is -X (-D -P --no-long-join --dual=no); strand="for" / "rev" is --for-only / --rev-only."""
+    is -X (-D -P --no-long-join --dual=no); strand="for" / "rev" is --for-only / --rev-only.  Spliced mapping: the presets
+    "splice", "splice:hq" and "cdna" (any "splice:..." is "splice"), splice=True is --splice (cDNA chaining on any preset),
+    max_intron_len=N is -G, applied after the preset and --splice; it changes nothing unless one of them set MM_F_SPLICE.
+    Spliced mapping has no base-level alignment: it needs cigar=False and sam=False."""
     L = _setup(lib())
     io, mo = IdxOpt(), MapOpt()
     L.wm_set_opt(None, C.byref(io), C.byref(mo))
     if preset is not None and L.wm_set_opt(preset.encode(), C.byref(io), C.byref(mo)) != 0:
         raise ValueError(f"unknown preset {preset}")
+    if splice:
+        mo.flag |= F_SPLICE
+    if max_intron_len is not None:
+        L.wm_mapopt_max_intron_len(C.byref(mo), int(max_intron_len))
+    if (mo.flag & F_SPLICE) and (sam or cigar):
+        raise ValueError("spliced base-level alignment (-c / -a with a splice preset or --splice) is not built: "
+                         "map with cigar=False and sam=False for approximate PAF")
     if sam:
         mo.flag |= F_OUT_SAM | F_CIGAR
     elif cigar:
@@ -118,10 +132,13 @@ class Mapper:
     part_bases is -I: the reference is cut into index parts of about that many bases (wm_index_build_parts), which stay on the
     GPU together; the output is then part-major, or, with split=True (--split-prefix), the parts' hits are merged per read
     in memory (no temporary file is written).  mid_occ_frac is -f: each index part gets its own mid_occ, selected on the
-    GPU from its occurrence counts."""
+    GPU from its occurrence counts.
+    preset="splice" / "splice:hq" / "cdna" with cigar=False maps spliced reads (approximate PAF, cDNA chaining); splice=True is
+    --splice and max_intron_len is -G (make_options)."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
-                 no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None):
+                 no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None,
+                 splice=False, max_intron_len=None):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
@@ -131,7 +148,8 @@ class Mapper:
         if mid_occ_frac is not None and not 0.0 <= mid_occ_frac < 1.0:
             raise ValueError(f"mid_occ_frac must be in [0, 1), not {mid_occ_frac!r}")
         self.L = _setup(lib())
-        self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand)
+        self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand,
+                                        splice=splice, max_intron_len=max_intron_len)
         if hpc:
             self.io.flag |= I_HPC
         if mid_occ_frac is not None:
