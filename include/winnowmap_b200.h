@@ -347,6 +347,12 @@ int wm_map_file(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, const char *reads_fn, c
                 int tag_order, int64_t max_batch_bases);
 /* the command line recorded in the @PG header line of SAM output (the reference prints its own argv, src/format.c:130-135) */
 void wm_set_sam_cl(wm_gpu_ctx *ctx, const char *cl);
+/* The winnowmap command line (src/main.c): `winnowmap [options] ref.fa reads.fa [...]` with the reference's options, output
+ * and exit statuses, mapped on device 0.  The index is built from ref.fa (and -W), cut into parts under -I; every query
+ * file is mapped part by part in argument order, or merged over the parts under --split-prefix.  Options the mapper does
+ * not build (--sr, --heap-sort=yes, -T > 0, --frag=yes, spliced base alignment) are refused with status 1 before any index
+ * is built.  @PG CL: records "winnowmap" and argv[1..].  Returns the exit status. */
+int wm_cli_main(int argc, char **argv);
 /* mm_gen_cs / mm_gen_MD (src/minimap.h:389-390): the cs / MD string of one hit of read `seq` (ASCII) into *buf, which is
  * realloc()ed when *max_len is too small; returns the length.  The reference sequence comes from the context's index. */
 int wm_gen_cs(const wm_gpu_ctx *ctx, char **buf, int *max_len, const wm_reg1_t *r, const char *seq, int no_iden);

@@ -7,6 +7,7 @@ import gzip
 import hashlib
 import json
 import os
+import shutil
 import subprocess
 import sys
 
@@ -731,8 +732,69 @@ def main_splice():
     json.dump(manifest, open(os.path.join(gdir, "splice_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# The command line (winnowmap_b200/winnowmap-b200, tests/test_cli_host.py, tests/test_gpu_cli.py): reference runs on inputs
+# written under fixed relative names (ref.fa, reads.fa, reads_a.fa + reads_b.fa: the reads split in two files, rep.txt), run
+# from their directory so that the @PG CL: of the SAM header is stable.  {W} stands for "-W rep.txt" where the input has a list.
+CLI_CASES = {
+    "cli_sv_cap50M": dict(inputs="ont_sv", args="-t 4 -c -x map-ont --cap-sw-mem 50M {W} ref.fa reads.fa"),
+    "cli_sv_cap5M": dict(inputs="ont_sv", args="-t 4 -c -x map-ont --cap-sw-mem 5M {W} ref.fa reads.fa"),
+    "cli_sv_maxqlen": dict(inputs="ont_sv", args="-t 4 -c -x map-ont --max-qlen 8000 {W} ref.fa reads.fa"),
+    "cli_small_rg": dict(inputs="ont_small", args="-t 4 -a -x map-ont -R @RG\\tID:rg1\\tSM:s1 {W} ref.fa reads.fa"),
+    "cli_two_files_paf": dict(inputs="ont_small", args="-t 4 -c -x map-ont {W} ref.fa reads_a.fa reads_b.fa"),
+    "cli_two_files_sam": dict(inputs="ont_small", args="-t 4 -a -x map-ont {W} ref.fa reads_a.fa reads_b.fa"),
+    "cli_parts_two_files": dict(inputs="ont_tandem", args="-t 4 -c -x map-ont -I 330k {W} ref.fa reads_a.fa reads_b.fa"),
+}
+
+
+def make_cli_inputs(inputs, outdir):
+    """The files of a command-line case under their fixed names in outdir."""
+    os.makedirs(outdir, exist_ok=True)
+    tmp = os.path.join(outdir, "gen")
+    ref, reads, wfile = make_inputs(inputs, tmp)
+    shutil.copy(ref, os.path.join(outdir, "ref.fa"))
+    shutil.copy(reads, os.path.join(outdir, "reads.fa"))
+    recs = read_fasta(reads)
+    for half, part in (("a", recs[: len(recs) // 2]), ("b", recs[len(recs) // 2:])):
+        with open(os.path.join(outdir, f"reads_{half}.fa"), "w") as f:
+            for nm, sq in part:
+                f.write(f">{nm}\n{sq}\n")
+    if wfile:
+        shutil.copy(wfile, os.path.join(outdir, "rep.txt"))
+    return wfile is not None
+
+
+def cli_args(name, has_w):
+    """argv[1..] of a case (no argument holds a space)"""
+    return CLI_CASES[name]["args"].replace("{W}", "-W rep.txt" if has_w else "").split()
+
+
+def cli_golden_bytes(out, sam):
+    """What is committed of a run's output: PAF as it is, SAM with SEQ and QUAL replaced by their lengths."""
+    return sam_strip_seq(out) if sam else out
+
+
+def main_cli():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    gdir = os.path.join(ROOT, "tests", "golden")
+    manifest = {}
+    for name in CLI_CASES:
+        td = os.path.join("/tmp/wm_golden_cli", name)
+        has_w = make_cli_inputs(CLI_CASES[name]["inputs"], td)
+        args = cli_args(name, has_w)
+        out = subprocess.run([refbin] + args, cwd=td, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+        sam = "-a" in args
+        with gzip.GzipFile(os.path.join(gdir, name + (".sam.stripped.gz" if sam else ".paf.gz")), "wb", mtime=0) as f:
+            f.write(cli_golden_bytes(out, sam))
+        manifest[name] = dict(CLI_CASES[name], sam=sam, cmd=" ".join(["winnowmap"] + args), ref_md5=md5(os.path.join(td, "ref.fa")),
+                              reads_md5=md5(os.path.join(td, "reads.fa")), n_lines=out.count(b"\n"), out_md5=hashlib.md5(out).hexdigest())
+        print(name, manifest[name]["n_lines"], "lines")
+    json.dump(manifest, open(os.path.join(gdir, "cli_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
-    if "--splice" in sys.argv:
+    if "--cli" in sys.argv:
+        main_cli()
+    elif "--splice" in sys.argv:
         main_splice()
     elif "--hpc" in sys.argv:
         main_hpc()

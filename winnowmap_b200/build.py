@@ -1,5 +1,6 @@
 """Builds winnowmap_b200/libwinnowmap_b200.so (CUDA kernels + C ABI) in-tree with nvcc for
-sm_90a (H100).  No JIT cache: the .so is built once by build() and loaded from the tree."""
+sm_90a (H100), and next to it the command-line executable winnowmap_b200/winnowmap-b200, which finds the .so through an
+$ORIGIN rpath.  No JIT cache: both are built once by build() and loaded from the tree."""
 import glob
 import os
 import subprocess
@@ -8,6 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libwinnowmap_b200.so")
+EXE = os.path.join(HERE, "winnowmap-b200")
+EXE_SRC = os.path.join(HERE, "cli", "main.c")
 NVCC = os.environ.get("WM_NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # -fmad=false: the reference is built without FMA contraction (Makefile:4); chaining and the
@@ -21,7 +24,7 @@ def sources():
 
 
 def needs_build():
-    if not os.path.exists(SO):
+    if not os.path.exists(SO) or not os.path.exists(EXE) or os.path.getmtime(EXE) < max(os.path.getmtime(SO), os.path.getmtime(EXE_SRC)):
         return True
     t = os.path.getmtime(SO)
     deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + \
@@ -56,7 +59,14 @@ def build(force=False, verbose=False):
         sys.stderr.write("\n".join(log))
     cmd = [NVCC] + ARCH + ["-shared", "-o", SO] + objs + ["-ccbin", "/usr/bin/g++", "-lpthread", "-lz", "-lgomp"]
     subprocess.check_call(cmd)
+    build_exe()
     return SO
+
+
+def build_exe():
+    """winnowmap_b200/winnowmap-b200: main() only calls wm_cli_main of the .so beside it"""
+    subprocess.check_call(["/usr/bin/gcc", "-O2", "-I", os.path.join(HERE, "..", "include"), EXE_SRC, "-o", EXE, "-L", HERE,
+                           "-lwinnowmap_b200", "-Wl,-rpath,$ORIGIN"])
 
 
 if __name__ == "__main__":

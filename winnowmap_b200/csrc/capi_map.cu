@@ -16,6 +16,7 @@
 #include "topfreq.cuh"
 #include "occ_select.cuh"
 #include "gpu_backend.h"
+#include "host_cli.h"
 #include "host_driver.h"
 #include "host_io.h"
 #include "host_index.h"
@@ -646,6 +647,23 @@ extern "C" int wm_map_file(wm_gpu_ctx_s *c, const wm_mapopt_t *opt, const char *
 }
 
 extern "C" void wm_set_sam_cl(wm_gpu_ctx_s *c, const char *cl) { c->sam_cl = cl ? cl : ""; }
+
+// The winnowmap command line (host_cli.h) over an index built on device 0, cut into parts under -I
+extern "C" int wm_cli_main(int argc, char **argv)
+{
+	struct OwnedParts : CtxParts {
+		explicit OwnedParts(wm_gpu_ctx_s *c) : CtxParts(c) {}
+		~OwnedParts() override { wm_gpu_destroy(c); }
+	};
+	return cli_main(argc, argv, [](const CliArgs &a) -> std::unique_ptr<IndexParts> {
+		require_device("winnowmap-b200");
+		wm_idxopt_t io = a.ipt;
+		io.flag &= WM_I_HPC; // the other index flags only drop what a prebuilt index stores
+		wm_gpu_ctx_s *c = wm_index_build_parts(a.files[0].c_str(), a.has_kmer ? a.kmer_fn.c_str() : 0, &io, 0.0, 0);
+		if (!c) return nullptr;
+		return std::unique_ptr<IndexParts>(new OwnedParts(c));
+	});
+}
 
 // mm_gen_cs / mm_gen_MD (src/minimap.h:389-390, src/format.c:245-266): *buf is (re)allocated with realloc() when it is too
 // small, *max_len is its capacity; the string is NUL terminated; returns its length

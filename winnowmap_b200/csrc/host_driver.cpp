@@ -15,12 +15,12 @@
 namespace wmh {
 
 void format_read(std::string &dst, const wm_host_idx *mi, int64_t opt_flag, const wm_read *t, int n_reg, const wm_reg1_t *regs, int rep_len,
-                 const char *prefix)
+                 const char *prefix, const char *rg_id)
 {
 	std::string line;
 	const bool sam = (opt_flag & WM_F_OUT_SAM) != 0;
 	auto emit = [&](int j) { // hit j of the read, or the empty record (j < 0)
-		if (sam) write_sam(line, mi, t, j, n_reg, regs, opt_flag, rep_len, "");
+		if (sam) write_sam(line, mi, t, j, n_reg, regs, opt_flag, rep_len, rg_id ? rg_id : "");
 		else write_paf(line, mi, t, j >= 0 ? &regs[j] : 0, opt_flag, rep_len);
 		if (prefix) dst += prefix;
 		dst += line; dst += '\n';
@@ -72,12 +72,12 @@ bool map_merged(IndexParts &ix, const wm_mapopt_t *opt, const std::vector<const 
 // One pass over the read file: part `part` of ix (mapped and written as mm_map_file does), or, with part < 0, every part
 // mapped and merged per read (map_merged), written with the sequence table of all parts.  Reads are taken in the reference's
 // mini-batches (src/bseq.c:80-119), sorted by length descending inside a batch (src/map.c:1124-1143) and printed in that
-// order (:1173-1208).
-static int map_file_pass(IndexParts &ix, int part, const wm_mapopt_t *opt_in, const char *reads_fn, FILE *out, int n_threads, int rank, int world,
-                         int tag_order, int64_t max_batch_bases)
+// order (:1173-1208).  -2 when the read file cannot be opened.
+static int map_file_pass(IndexParts &ix, int part, const wm_mapopt_t *opt_in, const char *reads_fn, FILE *out, const char *rg_id, int n_threads, int rank,
+                         int world, int tag_order, int64_t max_batch_bases)
 {
 	SeqReader rd;
-	if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
+	if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -2; }
 	const bool merged = part < 0;
 	wm_mapopt_t opt_part;
 	if (!merged && !ix.part_opt(part, opt_in, &opt_part)) return -1;
@@ -129,7 +129,7 @@ static int map_file_pass(IndexParts &ix, int part, const wm_mapopt_t *opt_in, co
 			for (int i = 0; i < n; ++i) {
 				char tag[64];
 				if (tag_order) snprintf(tag, sizeof(tag), "%lld\t%d\t", (long long)b->no, b->mine_pos[i]);
-				format_read(lines[i], mi, opt->flag, b->mine[i], (int)b->regs[i].size(), b->regs[i].data(), b->rl[i], tag_order ? tag : 0);
+				format_read(lines[i], mi, opt->flag, b->mine[i], (int)b->regs[i].size(), b->regs[i].data(), b->rl[i], tag_order ? tag : 0, rg_id);
 				for (auto &rr : b->regs[i]) free(rr.p);
 			}
 			for (int i = 0; i < n; ++i) fwrite(lines[i].data(), 1, lines[i].size(), out);
@@ -173,34 +173,46 @@ static int map_file_pass(IndexParts &ix, int part, const wm_mapopt_t *opt_in, co
 // split_prefix the parts' hits are merged per read in one pass (mm_split_merge, src/map.c:1278-1321), also for a single
 // index: its @SQ lines then come twice, the normal header's and the merge's, as the reference prints them.  The reference
 // goes through temporary files <prefix>.NNNN.tmp; here the merge runs in memory and no file is written.
-int map_file(IndexParts &ix, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, const char *sam_cl, int n_threads, int rank, int world,
-             int tag_order, int64_t max_batch_bases)
+int map_files(IndexParts &ix, const wm_mapopt_t *opt, const std::vector<const char*> &reads_fns, const char *out_fn, const char *sam_cl, const char *rg,
+              int n_threads, int rank, int world, int tag_order, int64_t max_batch_bases)
 {
 	const bool merged = opt->split_prefix != 0;
 	if (ix.n_parts() > 1 && !merged && world > 1) {
 		fprintf(stderr, "[ERROR] wm_map_file: a multi-part index without split_prefix is written part-major, which does not shard over ranks\n");
 		return -1;
 	}
-	{ // the read file is checked before the output is created
-		SeqReader rd;
-		if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
-	}
 	FILE *out = out_fn && strcmp(out_fn, "-") ? fopen(out_fn, "wb") : stdout;
 	if (!out) return -1;
+	std::string rg_line, rg_id;
+	if ((opt->flag & WM_F_OUT_SAM) && rg && sam_rg_line(rg, rg_line, rg_id) < 0) rg_line.clear(), rg_id.clear(); // reported; mapping goes on
 	if ((opt->flag & WM_F_OUT_SAM) && rank == 0 && !tag_order) { // mm_write_sam_hdr (src/main.c:391-398); the merge's @SQ lines follow (src/map.c:1304-1306)
 		std::string h;
 		wm_host_idx none;
 		const wm_host_idx *all = ix.all();
-		write_sam_hdr(h, ix.n_parts() > 1 ? &none : all, "2.03", sam_cl);
+		write_sam_hdr(h, ix.n_parts() > 1 ? &none : all, "2.03", sam_cl, rg_line.empty() ? 0 : rg_line.c_str());
 		if (merged)
 			for (size_t i = 0; i < all->name.size(); ++i) { h += "@SQ\tSN:"; h += all->name[i]; h += "\tLN:"; h += std::to_string(all->len[i]); h += '\n'; }
 		fwrite(h.data(), 1, h.size(), out);
 	}
 	int rc = 0;
-	if (merged) rc = map_file_pass(ix, -1, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases);
-	else for (int p = 0; p < ix.n_parts() && rc == 0; ++p) rc = map_file_pass(ix, p, opt, reads_fn, out, n_threads, rank, world, tag_order, max_batch_bases);
+	auto pass = [&](int p, const char *fn) {
+		const int r = map_file_pass(ix, p, opt, fn, out, rg_id.c_str(), n_threads, rank, world, tag_order, max_batch_bases);
+		if (r == -1) rc = -1;
+	};
+	if (merged) for (size_t f = 0; f < reads_fns.size() && rc == 0; ++f) pass(-1, reads_fns[f]);
+	else for (int p = 0; p < ix.n_parts() && rc == 0; ++p) for (size_t f = 0; f < reads_fns.size() && rc == 0; ++f) pass(p, reads_fns[f]);
 	if (out != stdout) fclose(out); else fflush(out);
 	return rc;
+}
+
+int map_file(IndexParts &ix, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, const char *sam_cl, int n_threads, int rank, int world,
+             int tag_order, int64_t max_batch_bases)
+{
+	{ // the read file is checked before the output is created
+		SeqReader rd;
+		if (!rd.open(reads_fn)) { fprintf(stderr, "ERROR: failed to open file '%s': %s\n", reads_fn, strerror(errno)); return -1; }
+	}
+	return map_files(ix, opt, std::vector<const char*>(1, reads_fn), out_fn, sam_cl, 0, n_threads, rank, world, tag_order, max_batch_bases);
 }
 
 } // namespace wmh

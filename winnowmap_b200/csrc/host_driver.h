@@ -45,8 +45,9 @@ public:
 
 // The output step of one read (src/map.c:1189-1206): its hits as PAF or SAM lines (opt_flag says which), appended to dst.
 // prefix (if not null) starts every line.
+// rg_id is the @RG ID the SAM records carry ("" or null: none).
 void format_read(std::string &dst, const wm_host_idx *mi, int64_t opt_flag, const wm_read *t, int n_reg, const wm_reg1_t *regs, int rep_len,
-                 const char *prefix = 0);
+                 const char *prefix = 0, const char *rg_id = 0);
 
 // --split-prefix: every read mapped against every part, then merge_hits (src/map.c:1050-1105).  false when a part's options
 // are refused.
@@ -59,5 +60,13 @@ bool map_merged(IndexParts &ix, const wm_mapopt_t *opt, const std::vector<const 
 // 0, or -1 after an error.
 int map_file(IndexParts &ix, const wm_mapopt_t *opt, const char *reads_fn, const char *out_fn, const char *sam_cl, int n_threads, int rank, int world,
              int tag_order, int64_t max_batch_bases);
+
+// The loop of the reference's main() over the parts and the query files (src/main.c:384-424): the SAM header once, then part
+// by part every file in argument order (or, with split_prefix, every file merged over all parts).  rg is the -R line
+// (null: none), checked and unescaped as sam_write_rg_line does; under SAM its ID tags every record.  A query file that
+// cannot be opened is reported and skipped, as mm_map_file skips it.  The rest as map_file, which is this call with one file
+// that is checked before the output is created.
+int map_files(IndexParts &ix, const wm_mapopt_t *opt, const std::vector<const char*> &reads_fns, const char *out_fn, const char *sam_cl, const char *rg,
+              int n_threads, int rank, int world, int tag_order, int64_t max_batch_bases);
 
 } // namespace wmh

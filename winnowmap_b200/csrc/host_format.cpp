@@ -283,14 +283,34 @@ void write_sam(std::string &s, const wm_host_idx *mi, const wm_read *t, int reg_
 	if ((opt_flag & WM_F_COPY_COMMENT) && !t->comment.empty()) { s.push_back('\t'); s += t->comment; }
 }
 
-// mm_write_sam_hdr (src/format.c:118-139) without a read group: @SQ lines and the @PG line; `cl` is the command
-// line the caller wants recorded (the reference prints its own argv), may be null
-void write_sam_hdr(std::string &s, const wm_host_idx *mi, const char *version, const char *cl)
+int sam_rg_line(const char *s, std::string &line, std::string &id)
+{
+	line.clear(), id.clear();
+	if (strncmp(s, "@RG", 3) != 0) { fprintf(stderr, "[ERROR] the read group line is not started with @RG\n"); return -1; }
+	if (strchr(s, '\t')) { fprintf(stderr, "[ERROR] the read group line contained literal <tab> characters -- replace with escaped tabs: \\t\n"); return -1; }
+	for (const char *p = s; *p; ++p) { // mm_escape (src/format.c:68-80): \t and \\ resolved, any other escape dropped
+		if (*p != '\\') { line.push_back(*p); continue; }
+		if (!*++p) break;
+		if (*p == 't') line.push_back('\t');
+		else if (*p == '\\') line.push_back('\\');
+	}
+	const size_t at = line.find("\tID:");
+	if (at == std::string::npos) { fprintf(stderr, "[ERROR] no ID within the read group line\n"); line.clear(); return -1; }
+	const size_t b = at + 4, e = line.find_first_of("\t\n", b);
+	id = line.substr(b, e == std::string::npos ? std::string::npos : e - b);
+	if (id.size() + 1 > 256) { fprintf(stderr, "[ERROR] @RG:ID is longer than 255 characters\n"); line.clear(), id.clear(); return -1; }
+	return 0;
+}
+
+// mm_write_sam_hdr (src/format.c:118-139): @SQ lines, the read group line and the @PG line; `cl` is the command line the
+// caller wants recorded (the reference prints its own argv), may be null
+void write_sam_hdr(std::string &s, const wm_host_idx *mi, const char *version, const char *cl, const char *rg_line)
 {
 	s.clear();
 	for (size_t i = 0; i < mi->name.size(); ++i) {
 		s += "@SQ\tSN:"; s += mi->name[i]; s += "\tLN:"; put_int(s, (int)mi->len[i]); s.push_back('\n');
 	}
+	if (rg_line) { s += rg_line; s.push_back('\n'); }
 	s += "@PG\tID:Winnowmap\tPN:Winnowmap";
 	if (version) { s += "\tVN:"; s += version; }
 	if (cl && cl[0]) { s += "\tCL:"; s += cl; }

@@ -32,7 +32,10 @@ void write_sam(std::string &s, const wm_host_idx *mi, const wm_read *t, int reg_
                const char *rg_id);
 // cs / MD difference string of one hit without the tag prefix (mm_gen_cs / mm_gen_MD, src/format.c:245-266); seq = the read, ASCII
 void gen_cs_or_MD(std::string &s, const wm_host_idx *mi, const wm_reg1_t *r, const char *seq, int is_MD, int no_iden);
-// @SQ and @PG header lines (mm_write_sam_hdr, src/format.c:118-139)
-void write_sam_hdr(std::string &s, const wm_host_idx *mi, const char *version, const char *cl);
+// @SQ, @RG and @PG header lines (mm_write_sam_hdr, src/format.c:118-139); rg_line is what sam_rg_line made of -R, or null
+void write_sam_hdr(std::string &s, const wm_host_idx *mi, const char *version, const char *cl, const char *rg_line = 0);
+// The read group of -R (sam_write_rg_line, src/format.c:82-116): the line with its \t and \\ escapes resolved, and its ID.
+// -1, with a message, when the line does not start with @RG, holds a literal tab, has no ID or an ID over 255 characters.
+int sam_rg_line(const char *s, std::string &line, std::string &id);
 
 } // namespace wmh

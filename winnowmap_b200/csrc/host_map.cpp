@@ -93,6 +93,28 @@ ChainParams chain_params(const wm_mapopt_t *o, const wm_mapopt_t *base, int qlen
 	return c;
 }
 
+// mm_align_pair skips a DP whose matrix has more than max_sw_mat cells (--cap-sw-mem, src/align.c:323-325): such a job is not
+// shipped, and its result is the reset ksw_extz_t, Z-dropped.  The alignment walk then goes on from it as the reference's does.
+void run_dp_capped(Backend *be, int64_t max_sw_mat, const std::vector<DpJob> &jobs, const std::vector<MapWin> &wins, const DpScoring &sc,
+                   std::vector<DpRes> &res)
+{
+	auto capped = [&](const DpJob &j) { return max_sw_mat > 0 && (int64_t)j.t.len * j.q.len > max_sw_mat; };
+	if (std::none_of(jobs.begin(), jobs.end(), capped)) { be->run_dp(jobs, wins, sc, res); return; }
+	std::vector<DpJob> sent;
+	std::vector<size_t> where;
+	for (size_t i = 0; i < jobs.size(); ++i)
+		if (!capped(jobs[i])) sent.push_back(jobs[i]), where.push_back(i);
+	std::vector<DpRes> got;
+	be->run_dp(sent, wins, sc, got);
+	DpRes z; // ksw_reset_extz (src/ksw2.h:153-158), then zdropped = 1
+	memset(&z, 0, sizeof(z));
+	z.max_q = z.max_t = z.mqe_t = z.mte_q = -1;
+	z.max = 0, z.score = z.mqe = z.mte = WM_KSW_NEG_INF;
+	z.zdropped = 1;
+	res.assign(jobs.size(), z);
+	for (size_t k = 0; k < where.size(); ++k) res[where[k]] = got[k];
+}
+
 } // namespace
 
 void set_name_order(wm_host_idx *mi)
@@ -149,10 +171,6 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		fprintf(stderr, "[ERROR] winnowmap-b200: max_occ > mid_occ (re-chaining of repetitive reads) is not implemented; the CLI cannot set it either (src/main.c:278)\n");
 		exit(1);
 	}
-	if (opt->max_qlen > 0) { // stage-1 / stage-2 length cut-off (src/map.c:356, :528, :725)
-		fprintf(stderr, "[ERROR] winnowmap-b200: max_qlen is not implemented\n");
-		exit(1);
-	}
 	if (opt->mid_occ_frac >= 0.0f && opt->mid_occ_frac < 1.0f) { // -f: the C ABI resolves it per index (wm_mapopt_update) before mapping
 		fprintf(stderr, "[ERROR] winnowmap-b200: mid_occ_frac (-f) reached the batch unresolved: set mid_occ from the index first (wm_mapopt_update)\n");
 		exit(1);
@@ -195,7 +213,8 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	for (int i = 0; i < n_reads; ++i) {
 		ReadState &R = rs[i];
 		R.qlen = (int)reads[i]->seq.size();
-		R.stage1 = opt2.SVaware && R.qlen >= opt2.SVawareMinReadLength && R.qlen > 0;
+		// a read longer than max_qlen skips stage 2 (src/map.c:725), so its stage-1 anchors would never be used
+		R.stage1 = opt2.SVaware && R.qlen >= opt2.SVawareMinReadLength && R.qlen > 0 && !(opt2.max_qlen > 0 && R.qlen > opt2.max_qlen);
 		if (!R.stage1) continue;
 		const int off = opt2.suffixSampleOffset;
 		const int n_start = 1 + (int)ceil(R.qlen * 1.0 / off); // src/map.c:304
@@ -205,6 +224,10 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 			Cursor c;
 			c.read = i, c.suffix_id = sb / off, c.sub_begin = sb >= R.qlen ? R.qlen - 1 : sb, c.step = 0, c.done = false;
 			for (int sub_len : levels) {
+				if (opt2.max_qlen > 0 && sub_len > opt2.max_qlen) { // the first window longer than max_qlen ends the start point (src/map.c:356, :528)
+					if (c.sub_begin + sub_len <= R.qlen || c.sub_begin - sub_len + 1 >= 0) break;
+					continue;
+				}
 				if (c.sub_begin + sub_len <= R.qlen) c.steps.push_back(std::make_pair(sub_len, 0));
 				if (c.sub_begin - sub_len + 1 >= 0) c.steps.push_back(std::make_pair(sub_len, 1));
 			}
@@ -311,7 +334,7 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 			g_timers.add("round.merge_jobs", Timers::now() - tm0);
 			if (active.empty()) break;
 			double t2 = now_s();
-			{ WM_TIMED("round.run_dp"); be->run_dp(dp_jobs, wins, sc, dp_res); }
+			{ WM_TIMED("round.run_dp"); run_dp_capped(be, opt->max_sw_mat, dp_jobs, wins, sc, dp_res); }
 			{ WM_TIMED("round.run_ll"); be->run_ll(ll_jobs, wins, sc, ll_res); }
 			t_dp_wave += now_s() - t2;
 			if (st) {
