@@ -228,8 +228,8 @@ typedef struct { /* mm_mapopt_t, src/minimap.h:112-176 */
 
 /* mm_set_opt / mm_check_opt (src/options.c:89,133): same presets, same return codes, plus -7 for two gap pairs whose
    int8 lanes in the reference's ksw_extd2_sse can wrap (-A + q + 2e > 128), which the device fill does not reproduce, and
-   -8 for MM_F_SPLICE together with MM_F_CIGAR: spliced mapping (splice, splice:hq, cdna, --splice) is built without its
-   base-level alignment.  mm_mapopt_max_intron_len (src/options.c:83-87, -G): max_gap_ref = bw = max_intron_len when
+   -8 for MM_F_SPLICE together with MM_F_CIGAR: spliced base-level alignment is a library / boundary path (wm_gpu_map_batch,
+   wm_map_file, wm_format_batch take such options and align); the command line refuses it until its refusal tests are retired.  mm_mapopt_max_intron_len (src/options.c:83-87, -G): max_gap_ref = bw = max_intron_len when
    MM_F_SPLICE is set and max_intron_len > 0, else nothing; apply it after the preset, as the CLI does. */
 int wm_set_opt(const char *preset, wm_idxopt_t *io, wm_mapopt_t *mo);
 int wm_check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo);
@@ -251,6 +251,10 @@ wm_gpu_ctx *wm_gpu_idx_upload(const wm_idx_view_t *idx, int device);
  * sketched homopolymer-compressed and the alignment anchors are adjusted as mm_adjust_minier does (src/align.c:350-365).
  * Any other bit is refused (NULL).  wm_gpu_idx_upload(idx, device) is wm_gpu_idx_upload_flag(idx, 0, device). */
 wm_gpu_ctx *wm_gpu_idx_upload_flag(const wm_idx_view_t *idx, int idx_flag, int device);
+/* Set in idx_flag by the caller when mm_idx_t::I holds junction intervals (--junc-bed, mm_idx_bed_read).  Junction annotation
+ * is not built: such a context maps, but spliced base-level alignment on it (MM_F_SPLICE | MM_F_CIGAR) is refused with a message
+ * and exit(1) instead of aligning without the intervals. */
+#define WM_IDX_JUNC 0x100
 /* the index flag the context maps with (MM_I_HPC or 0) */
 int wm_idx_flag(const wm_gpu_ctx *ctx);
 void wm_gpu_destroy(wm_gpu_ctx *ctx);
@@ -322,7 +326,8 @@ wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
  * MM_F_FOR_ONLY / MM_F_REV_ONLY (--for-only / --rev-only): the seed filter of skip_seed (src/map.c:132-154) runs on the
  * device.  Its name tests compare names[i] with the index's sequence names; names == NULL or names[i] == NULL is a read
  * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE maps with the cDNA chaining of the reference;
- * with MM_F_CIGAR it is refused (wm_check_opt's -8), as are MM_F_SR and MM_F_HEAP_SORT. */
+ * with MM_F_CIGAR it also aligns as mm_align_skeleton does for splice (ksw_exts2 on the device, both transcript strands per hit
+ * under MM_F_SPLICE_FOR | MM_F_SPLICE_REV, ts:A), without junction annotation.  MM_F_SR and MM_F_HEAP_SORT are refused. */
 int wm_gpu_map_batch(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, int n_seq, const char *const *names, const char *const *seqs,
                      const int32_t *lens, int32_t *n_reg, wm_reg1_t **reg, int32_t *rep_len, int32_t *frag_gap, int n_threads);
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Spliced mapping (-x splice -W, no base alignment) on a generated transcriptome (tools/gen_data.py make_transcriptome).
 
-  python tools/bench_splice.py [--genome 20000000] [--genes 600] [--reads 20000] [--threads N]
+  python tools/bench_splice.py [--genome 20000000] [--genes 600] [--reads 20000] [--threads N] [--align c|a]
 
 Prints one line per figure:
   map_file        Mapper.map_file rate over the whole read set, after a warm-up on a slice of it (GPU required; no CPU fallback)
@@ -10,6 +10,9 @@ Prints one line per figure:
                   same -W filter), how many tasks exceed the giant-task size (2048 anchors) and how many of their anchors have a
                   window (src/chain.c:49-55) that reaches more than 4096 anchors back, below the tile kernel's ring
   reference       the reference binary (oracle/_ref/winnowmap, when built) on the same inputs and thread count
+With --align c (or a), the runs are -c (or -a) through Mapper(..., spliced_alignment=True): the DP is ksw_exts2 on the GPU;
+map_file then also reports the number of DP and ll jobs, and the reference line whether the outputs are byte-identical (SAM:
+but for the @PG line).
 Everything is written to a temporary directory."""
 import argparse
 import ctypes as C
@@ -67,6 +70,7 @@ def main():
     ap.add_argument("--reads", type=int, default=20000)
     ap.add_argument("--threads", type=int, default=min(32, os.cpu_count() or 1))
     ap.add_argument("--sample", type=int, default=400)
+    ap.add_argument("--align", choices=("c", "a"), default=None)
     a = ap.parse_args()
     from winnowmap_b200 import lib
     from winnowmap_b200.mapper import Mapper
@@ -89,16 +93,20 @@ def main():
         print(f"device: {smi}")
     except Exception:
         print("device: nvidia-smi unavailable")
-    mp = Mapper(ref, wfile, preset="splice", cigar=False, n_threads=a.threads)
+    mp = Mapper(ref, wfile, preset="splice", cigar=a.align is not None, sam=a.align == "a", n_threads=a.threads, spliced_alignment=True)
+    out = os.path.join(td, "out.paf")
     mp.map_file(warm, os.path.join(td, "warm.paf"))
+    mp.reset_stats()
     L.wm_prof_enable(1); L.wm_prof_reset()
     t0 = time.perf_counter()
-    mp.map_file(reads, os.path.join(td, "out.paf"))
+    mp.map_file(reads, out)
     t = time.perf_counter() - t0
     prof = (C.c_double * 13)(); L.wm_prof_get(prof)
     L.wm_prof_enable(0)
-    n_lines = sum(1 for _ in open(os.path.join(td, "out.paf")))
-    print(f"map_file: {t:.2f} s, {bases / t / 1e6:.2f} Mbase/s, {n_lines} PAF lines")
+    n_lines = sum(1 for _ in open(out))
+    st = mp.stats()
+    print(f"map_file: {t:.2f} s, {bases / t / 1e6:.2f} Mbase/s, {n_lines} output lines"
+          + (f", {int(st['n_dp_jobs'])} DP jobs, {int(st['n_ll_jobs'])} ll jobs, DP rounds {st['t_dp']:.2f} s" if a.align else ""))
     ms_sum, ms_uni, n_l = prof[1 + 6], prof[2 + 6], prof[3 + 6]
     print(f"chain_kernels: {ms_uni if ms_uni > 0 else ms_sum:.1f} ms over {int(n_l)} launches ({ms_sum:.1f} ms summed over launches)")
     n_tasks, n_giant, n_ag, n_deep = giant_stats(ref, recs, wfile, a.sample, mp.io, mp.mo)
@@ -108,10 +116,15 @@ def main():
     refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
     if os.path.exists(refbin):
         t0 = time.perf_counter()
-        subprocess.run([refbin, "-t", str(a.threads), "-x", "splice", "-W", wfile, ref, reads], stdout=subprocess.DEVNULL,
-                       stderr=subprocess.DEVNULL, check=True)
+        got = subprocess.run([refbin, "-t", str(a.threads), "-x", "splice"] + (["-" + a.align] if a.align else []) + ["-W", wfile, ref, reads],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, check=True).stdout
         tr = time.perf_counter() - t0
         print(f"reference: {tr:.2f} s, {bases / tr / 1e6:.2f} Mbase/s with {a.threads} threads (index build included)")
+        if a.align:
+            import make_golden
+            mine = open(out, "rb").read()
+            same = make_golden.sam_without_pg(mine) == make_golden.sam_without_pg(got) if a.align == "a" else mine == got
+            print(f"identical: {same}")
     else:
         print("reference: oracle/_ref/winnowmap not built")
 

@@ -732,6 +732,58 @@ def main_splice():
     json.dump(manifest, open(os.path.join(gdir, "splice_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- spliced base-level alignment (-c / -a with -x splice / splice:hq / cdna or --splice): tests/golden/splice_aln_manifest.json
+# and splice_aln_*; the inputs of the splice_* cases.  The "tx" reads include unspliced genomic reads, whose two strand rounds tie
+# (trans_strand 3: no ts:A).  Library options: the MM_F_* bits the reference's options set / clear beyond -c / -a, -C, --cap-sw-mem.
+F_OUT_CS, F_OUT_MD, F_EQX, F_SOFTCLIP = 0x40, 0x1000000, 0x4000000, 0x80000
+F_SPLICE_FOR, F_SPLICE_REV, F_SPLICE_FLANK = 0x100, 0x200, 0x40000
+SPLICE_ALN_CASES = {
+    # name: (reads, reference options, library options)
+    "splice_aln_c": ("tx", ["-x", "splice", "-c"], dict(preset="splice")),
+    "splice_aln_a": ("tx", ["-x", "splice", "-a"], dict(preset="splice", sam=True)),
+    "splice_aln_hq_cs": ("tx_hq", ["-x", "splice:hq", "-c", "--cs"], dict(preset="splice:hq", set_flags=F_OUT_CS)),
+    "splice_aln_cdna_md": ("tx", ["-x", "cdna", "-a", "--MD"], dict(preset="cdna", sam=True, set_flags=F_OUT_MD)),
+    "splice_aln_eqx_Y": ("tx", ["-x", "splice", "-a", "--eqx", "-Y"], dict(preset="splice", sam=True, set_flags=F_EQX | F_SOFTCLIP)),
+    "splice_aln_uf": ("tx", ["-x", "splice", "-c", "-u", "f"], dict(preset="splice", set_flags=F_SPLICE_FOR, clear_flags=F_SPLICE_REV)),
+    "splice_aln_ur": ("tx", ["-x", "splice", "-c", "-u", "r"], dict(preset="splice", set_flags=F_SPLICE_REV, clear_flags=F_SPLICE_FOR)),
+    "splice_aln_un": ("tx", ["-x", "splice", "-c", "-u", "n"], dict(preset="splice", clear_flags=F_SPLICE_FOR | F_SPLICE_REV)),
+    "splice_aln_noflank": ("tx", ["-x", "splice", "-c", "--splice-flank=no"], dict(preset="splice", clear_flags=F_SPLICE_FLANK)),
+    "splice_aln_C3": ("tx", ["-x", "splice", "-c", "-C", "3"], dict(preset="splice", noncan=3)),
+    "splice_aln_H": ("tx", ["-x", "splice", "-c", "-H"], dict(preset="splice", hpc=True)),
+    "splice_aln_I_split": ("tx", ["-x", "splice", "-c", "-I", "500k", "--split-prefix", "SPLIT"],
+                           dict(preset="splice", part_bases=500000, split=True)),
+    "splice_aln_ont_long": ("tx_long", ["-x", "map-ont", "--splice", "-c"], dict(preset="map-ont", splice=True)),
+    "splice_aln_cap5M": ("tx", ["-x", "splice", "-c", "--cap-sw-mem", "5M"], dict(preset="splice", max_sw_mat=5000000)),
+    "splice_aln_G20k": ("tx", ["-x", "splice", "-c", "-G", "20000"], dict(preset="splice", max_intron_len=20000)),
+}
+
+
+def main_splice_aln():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_splice"
+    manifest = {}
+    for name, (reads_kind, args, lib_opts) in SPLICE_ALN_CASES.items():
+        ref, reads, wfile = make_splice_inputs(reads_kind, tmp)
+        args = [a if a != "SPLIT" else os.path.join(tmp, name + ".split") for a in args]
+        cmd = [refbin, "-t", "4"] + args + ["-W", wfile, ref, reads]
+        out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout
+        sam = "-a" in args
+        if sam:
+            out = sam_without_pg(out)
+        with gzip.GzipFile(os.path.join(gdir, name + (".sam.stripped.gz" if sam else ".paf.gz")), "wb", mtime=0) as f:
+            f.write(sam_strip_seq(out) if sam else out)
+        manifest[name] = dict(reads=reads_kind, lib=lib_opts, sam=sam, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile),
+                              # not "cmd": the command-line parse check replays every "cmd" of the manifests, and the
+                              # command line refuses spliced alignment
+                              ref_cmd=" ".join(["winnowmap"] + [a if not a.startswith(tmp) else "<prefix>" for a in cmd[1:-2]] + ["ref.fa", "reads.fa"]),
+                              out_md5=hashlib.md5(out).hexdigest(), n_lines=out.count(b"\n"))
+        print(name, manifest[name]["n_lines"], "lines")
+    json.dump(manifest, open(os.path.join(gdir, "splice_aln_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 # The command line (winnowmap_b200/winnowmap-b200, tests/test_cli_host.py, tests/test_gpu_cli.py): reference runs on inputs
 # written under fixed relative names (ref.fa, reads.fa, reads_a.fa + reads_b.fa: the reads split in two files, rep.txt), run
 # from their directory so that the @PG CL: of the SAM header is stable.  {W} stands for "-W rep.txt" where the input has a list.
@@ -794,6 +846,8 @@ def main_cli():
 if __name__ == "__main__":
     if "--cli" in sys.argv:
         main_cli()
+    elif "--splice-aln" in sys.argv:
+        main_splice_aln()
     elif "--splice" in sys.argv:
         main_splice()
     elif "--hpc" in sys.argv:

@@ -185,11 +185,11 @@ static bool idx_flag_ok(const char *who, int flag)
 extern "C" wm_gpu_ctx_s *wm_gpu_idx_upload_flag(const wm_idx_view_t *v, int idx_flag, int device)
 {
 	require_device("wm_gpu_idx_upload");
-	if (!kw_ok("wm_gpu_idx_upload", v->k, v->w) || !idx_flag_ok("wm_gpu_idx_upload", idx_flag)) return 0;
+	if (!kw_ok("wm_gpu_idx_upload", v->k, v->w) || !idx_flag_ok("wm_gpu_idx_upload", idx_flag & ~WM_I_JUNC)) return 0;
 	wm_gpu_ctx_s *c = new wm_gpu_ctx_s();
 	memset(&c->stats, 0, sizeof(c->stats));
 	c->device = device; c->t_index = c->t_map = 0;
-	c->hidx.k = v->k, c->hidx.w = v->w, c->hidx.flag = idx_flag;
+	c->hidx.k = v->k, c->hidx.w = v->w, c->hidx.flag = idx_flag & ~WM_I_JUNC, c->hidx.junc = (idx_flag & WM_I_JUNC) != 0;
 	for (int i = 0; i < v->n_seq; ++i) {
 		c->hidx.name.push_back(v->seq_name && v->seq_name[i] ? v->seq_name[i] : std::to_string(i));
 		c->hidx.len.push_back(v->seq_len[i]);

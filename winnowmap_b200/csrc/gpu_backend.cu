@@ -452,7 +452,12 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 	g.h_cig.clear();
 	if (n == 0) return;
 	wm_pkseq rd; rd.pk = (const uint32_t*)g.pk.p, rd.nm = (const uint32_t*)g.nm.p;
-	wm_dp_params P; wm_dp_params_init(&P, sc.mat, sc.q, sc.e, sc.q2, sc.e2);
+	wm_dp_params P;
+	if (sc.splice) wm_dp_params_init_splice(&P, sc.mat, sc.q, sc.e, sc.q2, sc.noncan, sc.junc_bonus);
+	else wm_dp_params_init(&P, sc.mat, sc.q, sc.e, sc.q2, sc.e2);
+	// a splice job is ksw_exts2: unbanded (w = -1), and its global state slice, when it needs one, is its own (wm_extd2_plan)
+	auto job_w = [&](const DpJob &J) { return sc.splice ? -1 : J.w; };
+	auto job_bytes = [&](const DpJob &J) { return wm_extd2_bt_bytes(J.q.len, J.t.len, job_w(J)) + (sc.splice ? wm_exts2_scratch_bytes(J.t.len) : 0); };
 	static int coop_on = -1; // WM_DP_COOP=0: every job on one warp (for comparison)
 	if (coop_on < 0) { const char *e = getenv("WM_DP_COOP"); coop_on = (e && *e == '0') ? 0 : 1; if (getenv("WM_DP_V1") && *getenv("WM_DP_V1") == '1') coop_on = 0; }
 	std::vector<int64_t> cig_base(n + 1, 0); // offsets into h_cig, by execution slot
@@ -467,7 +472,7 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 		size_t bt_bytes = 0; int end = done; int64_t cig_cap = 0, pool = 0; int max_tlen = 0, max_qlen = 0;
 		while (end < n) {
 			const DpJob &J = jobs[end];
-			size_t b = wm_extd2_bt_bytes(J.q.len, J.t.len, J.w);
+			size_t b = job_bytes(J);
 			if (end > done && bt_bytes + b > g.bt_budget) break;
 			bt_bytes += b; cig_cap += J.q.len + J.t.len + 2; pool += J.q.len + J.t.len; max_tlen = std::max(max_tlen, J.t.len); max_qlen = std::max(max_qlen, J.q.len);
 			++end;
@@ -498,7 +503,7 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 			// every sequence starts on a 16-byte boundary and is zero padded to one: the fill kernel stages it with bulk copies
 			joff[2 * i] = pool_off; pool_off += (J.q.len + 15) & ~15;
 			joff[2 * i + 1] = pool_off; pool_off += (J.t.len + 15) & ~15;
-			h_poff[i] = p_off; p_off += (int64_t)wm_extd2_bt_bytes(J.q.len, J.t.len, J.w);
+			h_poff[i] = p_off; p_off += (int64_t)wm_extd2_bt_bytes(J.q.len, J.t.len, job_w(J));
 			h_coff[i] = c_off; c_off += J.q.len + J.t.len + 2;
 			prof_bytes += 2.0 * (J.q.len + J.t.len) + 48; // SURVEY.md 8d: qlen + tlen (codes in) + (qlen + tlen) (traceback) + 48; C_block is counted on the device
 		}
@@ -510,13 +515,13 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 			D.q_off = joff[2 * i], D.t_off = joff[2 * i + 1];
 			gj[2 * i] = make_gather(g, J.q, wins[J.task], D.q_off);
 			gj[2 * i + 1] = make_gather(g, J.t, wins[J.task], D.t_off);
-			D.qlen = J.q.len, D.tlen = J.t.len, D.w = J.w, D.zdrop = J.zdrop, D.end_bonus = J.end_bonus, D.flag = J.flag;
+			D.qlen = J.q.len, D.tlen = J.t.len, D.w = job_w(J), D.zdrop = J.zdrop, D.end_bonus = J.end_bonus, D.flag = J.flag;
 			D.p_off = h_poff[i];
 			D.cig_off = h_coff[i]; D.cig_cap = J.q.len + J.t.len + 2; D.pad = -1;
 		}
-		const wm_extd2_plan_t plan = wm_extd2_plan(dj.data(), m, P.single != 0);
-		std::vector<int32_t> coop; // the big jobs go to the CTA-cooperative sweep (not for the single-affine and first-generation paths)
-		if (!P.single && coop_on)
+		const wm_extd2_plan_t plan = wm_extd2_plan(dj.data(), m, P.single != 0, P.splice != 0);
+		std::vector<int32_t> coop; // the big jobs go to the CTA-cooperative sweep (not for the single-affine, splice and first-generation paths)
+		if (!P.single && !P.splice && coop_on)
 			for (int i = 0; i < m && dj[i].qlen + dj[i].tlen >= 1600; ++i) // (sorted by qlen + tlen, descending)
 				if (dj[i].pad >= 0 && wm_dp_is_coop(dj[i].qlen, dj[i].tlen, dj[i].w)) { dj[i].flag |= WM_DP_COOP; coop.push_back(i); }
 		g_timers.add("dp.host_prep", Timers::now() - tp0);
@@ -550,7 +555,11 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 		int64_t *d_joff = (int64_t*)g.g_joff.need(sizeof(int64_t) * joff.size());
 		uint8_t *d_pool = (uint8_t*)g.seq_pool.need(pool_off + 16);
 		wm_dp_job *d_dj = (wm_dp_job*)g.dp_jobs.need(sizeof(wm_dp_job) * m);
-		uint8_t *d_bt = (uint8_t*)g.bt.need(p_off + 16);
+		// a splice launch's state slices sit behind the traceback matrices in the same buffer: what run_dp counted against
+		// bt_budget per chunk is one allocation, so the buffer's size follows the budget and not the sum of two high-water marks
+		const size_t bt_end = ((size_t)p_off + 15) / 16 * 16;
+		uint8_t *d_bt = (uint8_t*)g.bt.need(bt_end + (P.splice ? plan.splice_bytes : 0) + 16);
+		int8_t *d_scr = P.splice ? (int8_t*)(d_bt + bt_end) : 0;
 		wm_extz_dev *d_ez = (wm_extz_dev*)g.ez.need(sizeof(wm_extz_dev) * m);
 		uint32_t *d_cig = (uint32_t*)g.cig.need(sizeof(uint32_t) * (c_off + 1));
 		WM_CUDA_CHECK(wm_memcpy_async(d_gj, gj.data(), sizeof(wm_gather_job) * gj.size(), cudaMemcpyHostToDevice, st));
@@ -568,7 +577,7 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 			d_coop = (int32_t*)g.coop_ids.need(sizeof(int32_t) * coop.size());
 			WM_CUDA_CHECK(wm_memcpy_async(d_coop, coop.data(), sizeof(int32_t) * coop.size(), cudaMemcpyHostToDevice, st));
 		}
-		wm_extd2_launch(&g.dpws, d_dj, m, plan, d_pool, d_bt, d_ez, d_cig, P, st, &zp, d_zd, d_coop, (int)coop.size());
+		wm_extd2_launch(&g.dpws, d_dj, m, plan, d_pool, d_bt, d_ez, d_cig, P, st, &zp, d_zd, d_coop, (int)coop.size(), 0, d_scr);
 		// CIGAR lengths -> offsets -> compacted CIGARs, all behind the traceback on the stream: the host then only copies
 		int32_t *d_nc = (int32_t*)g.nc_buf.need(sizeof(int32_t) * (m + 1));
 		int64_t *d_ooff = (int64_t*)g.cig_off.need(sizeof(int64_t) * (m + 2));

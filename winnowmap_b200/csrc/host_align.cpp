@@ -15,6 +15,9 @@ namespace wmh {
 #define EZ_SCAN_ZDROP 0x10000 // not a ksw2 flag: asks the backend for the mm_test_zdrop score walk over the result (DpRes::has_zd)
 #define EZ_EXTZ_ONLY  0x40
 #define EZ_REV_CIGAR  0x80
+#define EZ_SPLICE_FOR 0x100
+#define EZ_SPLICE_REV 0x200
+#define EZ_SPLICE_FLANK 0x400
 
 // seq_nt4_table (src/sketch.c:19-36): bytes 0..3 and ACGT/acgt (U/u as T) are bases, everything else 4
 struct Nt4Table {
@@ -371,6 +374,94 @@ void AlignTask::init(const wm_mapopt_t *opt_, const wm_host_idx *mi_, int task_i
 	gen_simple_mat(mat, (int8_t)opt->a, (int8_t)opt->b, (int8_t)opt->sc_ambi);
 	n_a = squeeze_a(regs, a); // :880
 	phase = 0; cur = 0; sub = 0; inv_job = -1;
+	const int64_t both = WM_F_SPLICE | WM_F_SPLICE_FOR | WM_F_SPLICE_REV;
+	n_round = (opt->flag & both) == both ? 2 : 1; // :884
+}
+
+// The mm_align1 instances of one hit (one, or one per strand flag), and the ll jobs of mm_fix_bad_ends_splice (:545-563):
+// mm_seed_ext_score (:523-543) of the first and of the last anchor, where the anchor is short for the gap that follows it.
+// The filter reads the anchors' positions and spans only, so its result is the same in both rounds.
+void AlignTask::start_rounds(const wm_reg1_t &r, Align1 *A, JobSink &sink)
+{
+	for (int k = 0; k < n_round; ++k) {
+		A[k] = Align1(); A[k].r = r; A[k].state = 0;
+		A[k].splice_flag = n_round == 2 ? (k == 0 ? WM_F_SPLICE_FOR : WM_F_SPLICE_REV) : (int32_t)(opt->flag & (WM_F_SPLICE_FOR | WM_F_SPLICE_REV));
+	}
+	if (!(opt->flag & WM_F_SPLICE) || (opt->flag & WM_F_NO_END_FLT) || r.cnt < 3) return;
+	const int ext_len = opt->anchor_ext_len;
+	for (int e = 0; e < 2; ++e) {
+		const wm_pair_t *p = &a[e == 0 ? r.as : r.as + r.cnt - 1], *nb = e == 0 ? p + 1 : p - 1;
+		const double log_gap = e == 0 ? log((int32_t)nb->x - (int32_t)p->x) : log((int32_t)p->x - (int32_t)nb->x);
+		if ((p->y >> 32 & 0xff) >= log_gap + opt->anchor_ext_shift) continue;
+		const int q_span = p->y >> 32 & 0xff, rid = (int)(p->x << 1 >> 33), ref_len = (int)mi->len[rid];
+		int re = (int)((uint32_t)p->x + 1), rs = re - q_span, qe = (int)((uint32_t)p->y + 1), qs = qe - q_span;
+		rs = rs - ext_len > 0 ? rs - ext_len : 0;
+		qs = qs - ext_len > 0 ? qs - ext_len : 0;
+		re = re + ext_len < ref_len ? re + ext_len : ref_len;
+		qe = qe + ext_len < qlen ? qe + ext_len : qlen;
+		LlJob j;
+		j.task = task_id;
+		j.q = SeqRef{ (int32_t)(p->x >> 63) ? SEQ_Q1 : SEQ_Q0, 0, qs, qe - qs, 0 };
+		j.t = SeqRef{ SEQ_REF, rid, rs, re - rs, 0 };
+		A[0].end_ll[e] = (int)sink.ll.size();
+		sink.ll.push_back(j);
+	}
+}
+
+// as1 / cnt1 of mm_fix_bad_ends_splice from the ll scores, then everything mm_align1 does before its first DP, per round
+void AlignTask::plan_rounds(Align1 *A, const LlRes *ll, JobSink &sink)
+{
+	if ((opt->flag & WM_F_SPLICE) && !(opt->flag & WM_F_NO_END_FLT)) {
+		const wm_reg1_t *r = &A[0].r;
+		int32_t as1 = r->as, cnt1 = r->cnt;
+		for (int e = 0; e < 2; ++e) {
+			if (A[0].end_ll[e] < 0) continue;
+			const wm_pair_t *p = &a[e == 0 ? r->as : r->as + r->cnt - 1], *nb = e == 0 ? p + 1 : p - 1;
+			const double log_gap = e == 0 ? log((int32_t)nb->x - (int32_t)p->x) : log((int32_t)p->x - (int32_t)nb->x);
+			if ((double)ll[A[0].end_ll[e]].score / mat[0] < log_gap + opt->anchor_ext_shift) { // "score < log_4(gap) + shift"
+				if (e == 0) ++as1;
+				--cnt1;
+			}
+		}
+		for (int k = 0; k < n_round; ++k) A[k].end_as1 = as1, A[k].end_cnt1 = cnt1, A[k].end_ll[0] = A[k].end_ll[1] = -1;
+	}
+	for (int k = 0; k < n_round; ++k) plan1(A[k], sink);
+}
+
+// The round a hit keeps (:890-904): the higher dp_score; on a tie trans_strand 3 and a choice by parity.  One round: the
+// strand flag says it, so `-u n` gives trans_strand 2.
+void AlignTask::pick_round(Align1 *A, wm_reg1_t *r, wm_reg1_t *r2) const
+{
+	auto extra = [](wm_reg1_t *x) { // (the reference dereferences p here; a hit without any DP has none)
+		if (x->p) return;
+		uint32_t capacity = round_up_pow2((uint32_t)(sizeof(wm_extra_t) / 4));
+		x->p = (wm_extra_t*)calloc(capacity, 4);
+		x->p->capacity = capacity;
+	};
+	if (n_round == 2) {
+		extra(&A[0].r), extra(&A[1].r);
+		int which, trans_strand;
+		if (A[0].r.p->dp_score > A[1].r.p->dp_score) which = 0, trans_strand = 1;
+		else if (A[0].r.p->dp_score < A[1].r.p->dp_score) which = 1, trans_strand = 2;
+		else trans_strand = 3, which = (qlen + A[0].r.p->dp_score) & 1;
+		*r = A[which].r, *r2 = A[which].r2;
+		free(A[!which].r.p);
+		r->p->trans_strand = trans_strand;
+		return;
+	}
+	*r = A[0].r, *r2 = A[0].r2;
+	if (opt->flag & WM_F_SPLICE) { extra(r); r->p->trans_strand = (opt->flag & WM_F_SPLICE_FOR) ? 1 : 2; }
+}
+
+// extra_flag of mm_align1 (:602-606): the splice signals of the round's strand flag, as seen from the hit's strand
+static int32_t ez_splice_flag(const wm_mapopt_t *opt, const Align1 &A)
+{
+	int32_t f = 0;
+	if (!(opt->flag & WM_F_SPLICE)) return 0;
+	if (A.splice_flag & WM_F_SPLICE_FOR) f |= A.rev ? EZ_SPLICE_REV : EZ_SPLICE_FOR;
+	if (A.splice_flag & WM_F_SPLICE_REV) f |= A.rev ? EZ_SPLICE_FOR : EZ_SPLICE_REV;
+	if (opt->flag & WM_F_SPLICE_FLANK) f |= EZ_SPLICE_FLANK;
+	return f;
 }
 
 static inline void adjust_minier(const wm_host_idx *mi, const uint8_t *const qseq0[2], const wm_pair_t *p, int32_t *r, int32_t *q)
@@ -410,8 +501,11 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 	const int bw = A.bw = (int)(opt->bw * 1.5 + 1.);
 	int32_t as1, cnt1, rs, qs, re, qe, rs0, qs0, re0, qe0, rs1, qs1, re1, qe1, i, l;
 	const int32_t ref_len = (int32_t)mi->len[rid];
-	if (!(opt->flag & WM_F_NO_END_FLT)) fix_bad_ends(r, a, opt->bw, opt->min_chain_score * 2, &as1, &cnt1);
-	else as1 = r->as, cnt1 = r->cnt;
+	if (!(opt->flag & WM_F_NO_END_FLT)) {
+		if (opt->flag & WM_F_SPLICE) as1 = A.end_as1, cnt1 = A.end_cnt1; // mm_fix_bad_ends_splice (plan_rounds)
+		else fix_bad_ends(r, a, opt->bw, opt->min_chain_score * 2, &as1, &cnt1);
+	} else as1 = r->as, cnt1 = r->cnt;
+	const int32_t extra_flag = ez_splice_flag(opt, A);
 	filter_bad_seeds(as1, cnt1, a, 10, 40, opt->max_gap >> 1, 10);
 	filter_bad_seeds_alt(as1, cnt1, a, 30, opt->max_gap >> 1);
 	adjust_minier(mi, q_strand, &a[as1], &rs, &qs);
@@ -485,7 +579,7 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 		j.q = SeqRef{ rev ? SEQ_Q1 : SEQ_Q0, 0, qs0, qs - qs0, 1 };
 		j.t = SeqRef{ SEQ_REF, rid, rs0, rs - rs0, 1 };
 		j.w = bw, j.end_bonus = opt->end_bonus, j.zdrop = r->split_inv ? opt->zdrop_inv : opt->zdrop;
-		j.flag = EZ_EXTZ_ONLY | EZ_RIGHT | EZ_REV_CIGAR;
+		j.flag = extra_flag | EZ_EXTZ_ONLY | EZ_RIGHT | EZ_REV_CIGAR;
 		A.left_job = (int)sink.dp.size();
 		sink.dp.push_back(j);
 	}
@@ -501,7 +595,7 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 			j.task = task_id;
 			j.q = SeqRef{ rev ? SEQ_Q1 : SEQ_Q0, 0, qs, qe - qs, 0 };
 			j.t = SeqRef{ SEQ_REF, rid, rs, re - rs, 0 };
-			j.w = g.bw1, j.end_bonus = -1, j.zdrop = opt->zdrop, j.flag = EZ_APPROX_MAX | EZ_SCAN_ZDROP; // first pass (:733)
+			j.w = g.bw1, j.end_bonus = -1, j.zdrop = opt->zdrop, j.flag = extra_flag | EZ_APPROX_MAX | EZ_SCAN_ZDROP; // first pass (:733)
 			g.job = (int)sink.dp.size();
 			sink.dp.push_back(j);
 			A.gaps.push_back(g);
@@ -515,7 +609,7 @@ void AlignTask::plan1(Align1 &A, JobSink &sink)
 		j.task = task_id;
 		j.q = SeqRef{ rev ? SEQ_Q1 : SEQ_Q0, 0, qe, qe0 - qe, 0 };
 		j.t = SeqRef{ SEQ_REF, rid, re, re0 - re, 0 };
-		j.w = bw, j.end_bonus = opt->end_bonus, j.zdrop = opt->zdrop, j.flag = EZ_EXTZ_ONLY;
+		j.w = bw, j.end_bonus = opt->end_bonus, j.zdrop = opt->zdrop, j.flag = extra_flag | EZ_EXTZ_ONLY;
 		A.right_job = (int)sink.dp.size();
 		sink.dp.push_back(j);
 	}
@@ -638,7 +732,7 @@ bool AlignTask::walk1(Align1 &A, const DpRes *dp, const LlRes *ll, JobSink &sink
 			j.task = task_id;
 			j.q = SeqRef{ rev ? SEQ_Q1 : SEQ_Q0, 0, g.qs, g.qe - g.qs, 0 };
 			j.t = SeqRef{ SEQ_REF, rid, g.rs, g.re - g.rs, 0 };
-			j.w = g.bw1, j.end_bonus = -1, j.zdrop = zdrop_code == 2 ? opt->zdrop_inv : opt->zdrop, j.flag = 0;
+			j.w = g.bw1, j.end_bonus = -1, j.zdrop = zdrop_code == 2 ? opt->zdrop_inv : opt->zdrop, j.flag = ez_splice_flag(opt, A);
 			A.pending_job = (int)sink.dp.size();
 			sink.dp.push_back(j);
 			A.zd_max_zdrop = zdrop_code;
@@ -690,6 +784,7 @@ bool AlignTask::walk1(Align1 &A, const DpRes *dp, const LlRes *ll, JobSink &sink
 		tbuf.resize(A.re1 > A.rs1 ? A.re1 - A.rs1 : 0);
 		if (A.re1 > A.rs1) mi->getseq(rid, A.rs1, A.re1, tbuf.data());
 		update_extra(r, qseq(r->rev) + A.qs1, tbuf.data(), mat, (int8_t)opt->q, (int8_t)opt->e, (int)(opt->flag & WM_F_EQX));
+		if (rev && r->p->trans_strand) r->p->trans_strand ^= 3; // :789-790, before mm_align_skeleton sets it
 		if (sub_t2) g_timers.add("adv.update_extra", Timers::now() - q0);
 	}
 	A.state = 9;
@@ -704,12 +799,26 @@ bool AlignTask::step_phase2(const DpRes *dp, const LlRes *ll, JobSink &sink)
 		if (cur >= out.size()) return true;
 		if (sub == 0) {
 			if (from_first[cur]) { sub = 4; }
-			else { child = Align1(); child.r = out[cur]; child.state = 0; plan1(child, sink); sub = 1; if (child.state != 9) return false; }
+			else {
+				start_rounds(out[cur], child, sink);
+				sub = 5;
+				if (ends_pending(child[0])) return false;
+			}
+		}
+		if (sub == 5) {
+			plan_rounds(child, ll, sink);
+			sub = 1;
+			bool planned = true;
+			for (int k = 0; k < n_round; ++k) if (child[k].state != 9) planned = false;
+			if (!planned) return false;
 		}
 		if (sub == 1) {
-			if (!walk1(child, dp, ll, sink)) return false;
-			out[cur] = child.r;
-			if (child.r2.cnt > 0) { out.insert(out.begin() + cur + 1, child.r2); from_first.insert(from_first.begin() + cur + 1, 0); }
+			bool done = true;
+			for (int k = 0; k < n_round; ++k) if (!walk1(child[k], dp, ll, sink)) done = false;
+			if (!done) return false;
+			wm_reg1_t r2;
+			pick_round(child, &out[cur], &r2);
+			if (r2.cnt > 0) { out.insert(out.begin() + cur + 1, r2); from_first.insert(from_first.begin() + cur + 1, 0); }
 			sub = 4;
 		}
 		if (sub == 4) { // inversion test against the element just before (:907-912)
@@ -802,8 +911,19 @@ bool AlignTask::advance(const DpRes *dp, const LlRes *ll, JobSink &sink)
 	static const bool sub_t = getenv("WM_SUBTIMING") != 0;
 	if (phase == 0) {
 		const double q0 = sub_t ? Timers::now() : 0;
-		firsts.resize(regs.size());
-		for (size_t i = 0; i < regs.size(); ++i) { firsts[i] = Align1(); firsts[i].r = regs[i]; firsts[i].state = 0; plan1(firsts[i], sink); }
+		firsts.resize(regs.size() * n_round);
+		bool wait = false;
+		for (size_t i = 0; i < regs.size(); ++i) {
+			start_rounds(regs[i], &firsts[i * n_round], sink);
+			wait = wait || ends_pending(firsts[i * n_round]);
+		}
+		phase = 4;
+		if (sub_t) g_timers.add("adv.phase0", Timers::now() - q0);
+		if (wait) return false;
+	}
+	if (phase == 4) {
+		const double q0 = sub_t ? Timers::now() : 0;
+		for (size_t i = 0; i < regs.size(); ++i) plan_rounds(&firsts[i * n_round], ll, sink);
 		phase = 1;
 		bool all = true;
 		for (auto &A : firsts) if (A.state != 9) all = false;
@@ -817,9 +937,11 @@ bool AlignTask::advance(const DpRes *dp, const LlRes *ll, JobSink &sink)
 		if (sub_t) g_timers.add("adv.walk1", Timers::now() - q0);
 		if (!all) return false;
 		out.clear(); from_first.clear();
-		for (auto &A : firsts) {
-			out.push_back(A.r); from_first.push_back(1);
-			if (A.r2.cnt > 0) { out.push_back(A.r2); from_first.push_back(0); }
+		for (size_t i = 0; i < firsts.size(); i += n_round) {
+			wm_reg1_t r, r2;
+			pick_round(&firsts[i], &r, &r2);
+			out.push_back(r); from_first.push_back(1);
+			if (r2.cnt > 0) { out.push_back(r2); from_first.push_back(0); }
 		}
 		firsts.clear();
 		phase = 2; cur = 0; sub = 0;

@@ -61,6 +61,11 @@ struct Align1 {
 	bool left_done, dropped;
 	int pending_job;        // job index of the outstanding ll / pass-2 request
 	int32_t zd_max_zdrop;   // carried across the ll round
+	// spliced alignment: the KSW_EZ_SPLICE_* bits of every DP of this instance (extra_flag, src/align.c:602-606), and the
+	// boundary-exon filter of mm_fix_bad_ends_splice (:545-563), planned once per hit and shared by its two strand rounds
+	int32_t splice_flag = 0;
+	int end_ll[2] = {-1, -1};   // ll job of the first / last anchor (mm_seed_ext_score), -1 if not needed
+	int32_t end_as1 = 0, end_cnt1 = 0;
 };
 
 struct AlignTask {
@@ -75,13 +80,14 @@ struct AlignTask {
 	int8_t mat[25];
 
 	// state
-	std::vector<Align1> firsts;  // phase 1: one per original hit, all in flight together
-	int phase;                   // 0 = init, 1 = phase 1 running, 2 = sequential follow-ups, 3 = finished
+	std::vector<Align1> firsts;  // phase 1: n_round per original hit, all in flight together
+	int n_round;                 // 2: spliced alignment with both strand flags (src/align.c:884-900), two mm_align1 per hit
+	int phase;                   // 0 = init, 4 = splice end filter planned, 1 = phase 1 running, 2 = sequential follow-ups, 3 = finished
 	// phase 2 (exact loop order of mm_align_skeleton for split children and inversions)
 	std::vector<wm_reg1_t> out;
 	size_t cur;                  // index into `out` of the element being processed
-	int sub;                     // 0 = need align1 (or reuse phase-1 result), 1 = align1 running, 2 = inv ll wait, 3 = inv dp wait
-	Align1 child;
+	int sub;                     // 0 = need align1 (or reuse phase-1 result), 5 = splice end filter wait, 1 = align1 running, 2 = inv ll wait, 3 = inv dp wait
+	Align1 child[2];
 	std::vector<char> from_first; // out[i] was aligned in phase 1
 	int inv_job; int32_t inv_ql, inv_tl, inv_qoff, inv_toff;
 
@@ -95,6 +101,10 @@ struct AlignTask {
 
 	const uint8_t *qseq(int strand) const { return q_strand[strand]; }
 private:
+	void start_rounds(const wm_reg1_t &r, Align1 *A, JobSink &sink);
+	bool ends_pending(const Align1 &A) const { return A.end_ll[0] >= 0 || A.end_ll[1] >= 0; }
+	void plan_rounds(Align1 *A, const LlRes *ll, JobSink &sink);
+	void pick_round(Align1 *A, wm_reg1_t *r, wm_reg1_t *r2) const;
 	void plan1(Align1 &A, JobSink &sink);
 	bool walk1(Align1 &A, const DpRes *dp, const LlRes *ll, JobSink &sink);
 	bool step_phase2(const DpRes *dp, const LlRes *ll, JobSink &sink);

@@ -52,7 +52,11 @@ struct SeedOut { // views into backend-owned host buffers, valid until the next 
 	int64_t n_b; const wm_pair_t *b;      // chained anchors, chains concatenated
 };
 
-struct DpScoring { int8_t mat[25]; int32_t q, e, q2, e2; };
+struct DpScoring {
+	int8_t mat[25]; int32_t q, e, q2, e2;
+	// spliced alignment (MM_F_SPLICE): every DP is ksw_exts2 (src/align.c:326-327) with q, e, q2, noncan and junc_bonus
+	int32_t splice = 0, noncan = 0, junc_bonus = 0;
+};
 
 class Backend {
 public:

@@ -277,7 +277,7 @@ int cli_parse(int argc, char **argv, CliArgs &a, int n_cpu)
 		                             "dual gap penalties violating E1>E2 and O1+E1<O2+E2", "--for-only and --rev-only can't be applied at the same time",
 		                             "-N must be no less than 0 and -p within 0 and 1", "-k and -w must be positive (k <= 28, w < 256), Z-drop not less than inversion Z-drop, and -X/-P not with --secondary=no",
 		                             "--cs or --MD doesn't work with --split-prefix", "dual gap penalties with -A + O1 + 2*E1 > 128 are not supported",
-		                             "spliced base-level alignment (-c, -a or --cs with -x splice, cdna or --splice) is not supported; map without them" };
+		                             "spliced base-level alignment (-c, -a or --cs with -x splice, cdna or --splice) is not supported by the command line: it is a library path (Mapper(spliced_alignment=True), wm_map_file)" };
 		fprintf(stderr, "[ERROR] %s\n", -rc < (int)(sizeof(msg) / sizeof(msg[0])) ? msg[-rc] : "invalid options");
 		return 1;
 	}

@@ -122,8 +122,8 @@ int check_opt(const wm_idxopt_t *io, const wm_mapopt_t *mo)
 	if ((mo->q != mo->q2 || mo->e != mo->e2) && mo->a + mo->q + 2 * mo->e > 128) return -7;
 	if (mo->zdrop < mo->zdrop_inv) return -5;
 	if ((mo->flag & WM_F_NO_PRINT_2ND) && (mo->flag & WM_F_ALL_CHAINS)) return -5;
-	// Not in the reference either: spliced mapping is built without its base-level alignment (the two-strand ksw_exts2 rounds of
-	// mm_align1 and ts:A), so splice with -c / -a is refused before any mapping instead of printing alignments that differ.
+	// Not in the reference: spliced base alignment (splice with -c / -a) is a library / boundary path (wm_gpu_map_batch,
+	// wm_map_file, Mapper(spliced_alignment=True)); the command line refuses it until its refusal tests are retired.
 	if ((mo->flag & WM_F_SPLICE) && (mo->flag & WM_F_CIGAR)) return -8;
 	return 0;
 }

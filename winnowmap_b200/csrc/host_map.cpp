@@ -162,8 +162,8 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		fprintf(stderr, "[ERROR] winnowmap-b200: sr/heap-sort modes are outside the accelerated path\n");
 		exit(1);
 	}
-	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR)) { // check_opt's -8: spliced mapping is built without base alignment
-		fprintf(stderr, "[ERROR] winnowmap-b200: spliced base-level alignment (splice with -c / -a) is not built; map without CIGAR\n");
+	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR) && mi->junc) { // mm_idx_bed_junc (src/index.c:780) is not built
+		fprintf(stderr, "[ERROR] winnowmap-b200: spliced base-level alignment with junction annotation (--junc-bed) is not supported\n");
 		exit(1);
 	}
 	// options the reference honours on this path that are not implemented here are refused, not silently ignored
@@ -197,6 +197,7 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	DpScoring sc;
 	gen_simple_mat(sc.mat, (int8_t)opt->a, (int8_t)opt->b, (int8_t)opt->sc_ambi);
 	sc.q = opt->q, sc.e = opt->e, sc.q2 = opt->q2, sc.e2 = opt->e2;
+	sc.splice = (opt->flag & WM_F_SPLICE) != 0, sc.noncan = opt->noncan, sc.junc_bonus = opt->junc_bonus;
 
 	std::vector<ReadState> rs(n_reads);
 	std::vector<uint32_t> skip(n_reads, 0), name_lt(n_reads, 0); // the seed filter of every read (-D, --dual=no, --for-only, --rev-only)

@@ -41,6 +41,7 @@
 #define WM_F_SAM_HIT_ONLY  0x40000000
 
 #define WM_I_HPC 0x1
+#define WM_I_JUNC WM_IDX_JUNC // not an mm_idx_t flag: the index carries junction intervals (mm_idx_t::I, --junc-bed)
 
 // anchor flag bits in mm128_t.y (src/mmpriv.h:17-23)
 #define WM_SEED_LONG_JOIN (1ULL << 40)
@@ -60,6 +61,7 @@ typedef wm128_t wm_pair_t; // mm128_t
 struct wm_host_idx {
 	int k, w;
 	int flag = 0;            // mm_idx_t::flag: WM_I_HPC when the index holds homopolymer-compressed minimizers
+	bool junc = false;       // the uploaded index carried junction intervals, which spliced alignment does not read (map_batch refuses)
 	std::vector<std::string> name;
 	std::vector<uint32_t> len;
 	std::vector<uint64_t> offset;

@@ -304,14 +304,29 @@ static int wm_use_v2(void)
 	return use_v2;
 }
 
+size_t wm_exts2_scratch_bytes(int tlen)
+{
+	const size_t b = (size_t)(tlen + 15) / 16 * 16 * WM_EXTS2_CELL_BYTES;
+	return b <= WM_FILL_SLICE ? 0 : b;
+}
+
 wm_extd2_plan_t wm_extd2_plan(wm_dp_job *h_jobs, int n, bool single, bool splice)
 {
-	wm_extd2_plan_t pl; pl.n_slots = 0, pl.max_tlen = 0, pl.max_qlen = 0;
-	const int use_v2 = single || splice ? 0 : wm_use_v2();
+	wm_extd2_plan_t pl; pl.n_slots = 0, pl.max_tlen = 0, pl.max_qlen = 0, pl.splice_bytes = 0;
+	if (splice) { // one slice per job, of the job's own size: J.pad counts WM_EXTS2_PAD_UNIT bytes
+		for (int i = 0; i < n; ++i) {
+			wm_dp_job &J = h_jobs[i];
+			const size_t b = wm_exts2_scratch_bytes(J.tlen);
+			J.pad = b == 0 ? -1 : (int32_t)(pl.splice_bytes / WM_EXTS2_PAD_UNIT);
+			pl.splice_bytes += b;
+		}
+		return pl;
+	}
+	const int use_v2 = single ? 0 : wm_use_v2();
 	for (int i = 0; i < n; ++i) {
 		wm_dp_job &J = h_jobs[i];
 		const int tlen16 = (J.tlen + 15) / 16 * 16;
-		const bool fits = splice ? (size_t)tlen16 * WM_EXTS2_CELL_BYTES <= WM_FILL_SLICE : use_v2 ? (tlen16 <= WM_V2_T && J.qlen <= WM_V2_Q) : tlen16 <= WM_SMEM_CELLS;
+		const bool fits = use_v2 ? (tlen16 <= WM_V2_T && J.qlen <= WM_V2_Q) : tlen16 <= WM_SMEM_CELLS;
 		J.pad = fits ? -1 : pl.n_slots++;
 		if (!fits) { if (J.tlen > pl.max_tlen) pl.max_tlen = J.tlen; if (J.qlen > pl.max_qlen) pl.max_qlen = J.qlen; }
 	}
@@ -329,16 +344,17 @@ cudaStream_t wm_stream_create_high_priority(void)
 
 void wm_extd2_launch(wm_extd2_ws *ws, const wm_dp_job *d_jobs, int n_jobs, const wm_extd2_plan_t &plan, const uint8_t *d_seq, uint8_t *d_bt,
                      wm_extz_dev *d_ez, uint32_t *d_cigar, const wm_dp_params &P, cudaStream_t stream, const wm_zd_params *zp, int32_t *d_zd,
-                     const int32_t *d_coop_ids, int n_coop, const uint8_t *d_junc)
+                     const int32_t *d_coop_ids, int n_coop, const uint8_t *d_junc, int8_t *d_scratch)
 {
 	if (n_jobs <= 0) return;
 	const size_t smem = (size_t)WM_FILL_WARPS * WM_FILL_SLICE;
 	const int use_v2 = P.single || P.splice ? 0 : wm_use_v2();
 	const int grid = (n_jobs + WM_FILL_WARPS - 1) / WM_FILL_WARPS;
-	// global state slices of the jobs that do not fit the shared-memory slice (wm_extd2_plan gave them slots)
+	// global state slices of the jobs that do not fit the shared-memory slice (wm_extd2_plan gave them slots; a splice job's
+	// slot is the offset of its own slice, in WM_EXTS2_PAD_UNIT bytes)
 	const int tcap = (plan.max_tlen + 15) / 16 * 16;
-	const size_t stride = plan.n_slots == 0 ? 0 : P.splice ? (size_t)tcap * WM_EXTS2_CELL_BYTES : use_v2 ? wm_v2_slice_bytes(tcap, plan.max_qlen) : (size_t)tcap * 11;
-	int8_t *gs = (int8_t*)ws->scratch.need(stride * (size_t)plan.n_slots + 16);
+	const size_t stride = P.splice ? WM_EXTS2_PAD_UNIT : plan.n_slots == 0 ? 0 : use_v2 ? wm_v2_slice_bytes(tcap, plan.max_qlen) : (size_t)tcap * 11;
+	int8_t *gs = d_scratch ? d_scratch : (int8_t*)ws->scratch.need((P.splice ? plan.splice_bytes : stride * (size_t)plan.n_slots) + 16);
 	if (!ws->fill_st) {
 		int lo = 0, hi = 0;
 		WM_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));

@@ -153,13 +153,18 @@ struct wm_extd2_ws {
 	wm_extd2_ws() : fill_st(0), coop_st(0), ev_ready(0), ev_done(0), ev_coop(0) {}
 	~wm_extd2_ws() { if (fill_st) { cudaStreamDestroy(fill_st); cudaStreamDestroy(coop_st); cudaEventDestroy(ev_ready); cudaEventDestroy(ev_done); cudaEventDestroy(ev_coop); } }
 };
-struct wm_extd2_plan_t { int n_slots, max_tlen, max_qlen; };
+struct wm_extd2_plan_t { int n_slots, max_tlen, max_qlen; size_t splice_bytes; }; // splice_bytes: the global slices of a splice launch
 void wm_dp_params_init(wm_dp_params *P, const int8_t *mat, int q, int e, int q2, int e2);
 void wm_dp_params_init_splice(wm_dp_params *P, const int8_t *mat, int q, int e, int q2, int noncan, int junc_bonus); // src/ksw2_exts2_sse.c:61-84
 size_t wm_extd2_bt_bytes(int qlen, int tlen, int w);
 // sets h_jobs[i].pad (global-scratch slot or -1) for the n jobs of one launch, in launch order; single: the jobs run the
 // single-affine sweep (wm_dp_params::single), whose state slice is 9 bytes per target cell
 wm_extd2_plan_t wm_extd2_plan(wm_dp_job *h_jobs, int n, bool single = false, bool splice = false); // splice: ksw_exts2.cuh, 12 bytes per cell
+// splice launches size every global slice by its own job: unbanded gap fills across introns reach 200 kb of target, and one
+// stride for all (the largest tlen) would multiply that by the number of jobs.  The global scratch a splice job of target
+// length tlen takes (0: it fits the shared-memory slice), a multiple of WM_EXTS2_PAD_UNIT.
+#define WM_EXTS2_PAD_UNIT 16
+size_t wm_exts2_scratch_bytes(int tlen);
 // Jobs flagged WM_DP_SCAN_ZDROP also get the score walk of mm_test_zdrop (src/align.c:32-70) over their CIGAR: five
 // int32 per job in d_zd (max_zdrop, t0, t1, q0, q1; max_zdrop = -1: no result).  zp / d_zd may be null.
 #define WM_DP_SCAN_ZDROP 0x10000
@@ -179,7 +184,8 @@ struct wm_zd_params { int32_t q, e; int8_t mat[25]; int8_t pad[3]; };
 void wm_extd2_launch(wm_extd2_ws *ws, const wm_dp_job *d_jobs, int n_jobs, const wm_extd2_plan_t &plan, const uint8_t *d_seq, uint8_t *d_bt,
                      wm_extz_dev *d_ez, uint32_t *d_cigar, const wm_dp_params &P, cudaStream_t stream,
                      const wm_zd_params *zp = 0, int32_t *d_zd = 0, const int32_t *d_coop_ids = 0, int n_coop = 0,
-                     const uint8_t *d_junc = 0); // d_junc: junction annotation parallel to d_seq (splice jobs), or null
+                     const uint8_t *d_junc = 0, int8_t *d_scratch = 0); // d_junc: junction annotation parallel to d_seq (splice jobs), or
+                     // null; d_scratch: the global state slices (plan.splice_bytes for a splice launch) from the caller, or null: ws->scratch
 cudaStream_t wm_stream_create_high_priority(void);
 // SMs of the current device: grids that hold a fixed number of CTAs per SM are sized from it
 static inline int wm_sm_count(void)

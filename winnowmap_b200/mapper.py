@@ -81,14 +81,28 @@ def _setup(L):
 F_OUT_SAM = 0x008
 
 
+E_SPLICE_CIGAR = -8  # wm_check_opt: MM_F_SPLICE together with MM_F_CIGAR
+
+
+def _check(L, io, mo, spliced_alignment):
+    rc = L.wm_check_opt(C.byref(io), C.byref(mo))
+    if rc == E_SPLICE_CIGAR and spliced_alignment:
+        return
+    if rc < 0:
+        raise ValueError(f"mm_check_opt-style validation failed: {rc}")
+
+
 def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, all_vs_all=False, strand=None, splice=False,
-                 max_intron_len=None):
+                 max_intron_len=None, spliced_alignment=False):
     """mm_set_opt(0) then mm_set_opt(preset) (reference main.c:144-159); -c sets MM_F_OUT_CG|MM_F_CIGAR, -a sets
     MM_F_OUT_SAM|MM_F_CIGAR (main.c).  Self and all-vs-all mapping: no_diag is -D, dual=False is --dual=no, all_vs_all
     is -X (-D -P --no-long-join --dual=no); strand="for" / "rev" is --for-only / --rev-only.  Spliced mapping: the presets
     "splice", "splice:hq" and "cdna" (any "splice:..." is "splice"), splice=True is --splice (cDNA chaining on any preset),
     max_intron_len=N is -G, applied after the preset and --splice; it changes nothing unless one of them set MM_F_SPLICE.
-    Spliced mapping has no base-level alignment: it needs cigar=False and sam=False."""
+    Spliced base-level alignment (-c / -a with spliced mapping: the two-strand ksw_exts2 rounds, ts:A, N in the CIGAR) is a
+    library path that has to be asked for: spliced_alignment=True accepts cigar / sam with spliced mapping, and the -8 that
+    wm_check_opt returns for that combination.  Without it, spliced mapping needs cigar=False and sam=False, as the command
+    line does until its refusal is lifted."""
     L = _setup(lib())
     io, mo = IdxOpt(), MapOpt()
     L.wm_set_opt(None, C.byref(io), C.byref(mo))
@@ -98,9 +112,9 @@ def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, a
         mo.flag |= F_SPLICE
     if max_intron_len is not None:
         L.wm_mapopt_max_intron_len(C.byref(mo), int(max_intron_len))
-    if (mo.flag & F_SPLICE) and (sam or cigar):
-        raise ValueError("spliced base-level alignment (-c / -a with a splice preset or --splice) is not built: "
-                         "map with cigar=False and sam=False for approximate PAF")
+    if (mo.flag & F_SPLICE) and (sam or cigar) and not spliced_alignment:
+        raise ValueError("spliced base-level alignment (-c / -a with a splice preset or --splice) is a library path: "
+                         "ask for it with spliced_alignment=True, or map with cigar=False and sam=False for approximate PAF")
     if sam:
         mo.flag |= F_OUT_SAM | F_CIGAR
     elif cigar:
@@ -115,9 +129,7 @@ def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, a
         if strand not in ("for", "rev", "both"):
             raise ValueError(f"strand must be 'for', 'rev' or 'both', not {strand!r}")
         mo.flag |= {"for": F_FOR_ONLY, "rev": F_REV_ONLY, "both": 0}[strand]
-    rc = L.wm_check_opt(C.byref(io), C.byref(mo))
-    if rc < 0:
-        raise ValueError(f"mm_check_opt-style validation failed: {rc}")
+    _check(L, io, mo, spliced_alignment)
     return io, mo
 
 
@@ -134,11 +146,13 @@ class Mapper:
     in memory (no temporary file is written).  mid_occ_frac is -f: each index part gets its own mid_occ, selected on the
     GPU from its occurrence counts.
     preset="splice" / "splice:hq" / "cdna" with cigar=False maps spliced reads (approximate PAF, cDNA chaining); splice=True is
-    --splice and max_intron_len is -G (make_options)."""
+    --splice and max_intron_len is -G (make_options).  With spliced_alignment=True they also align at base level (-c, or -a
+    with sam=True): ksw_exts2 on the GPU, both transcript strands tried per hit, ts:A, introns as N; the other flags of the
+    reference (--eqx, --cs, --MD, -u, --splice-flank, -C, --cap-sw-mem) are the fields of self.mo."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
                  no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None,
-                 splice=False, max_intron_len=None):
+                 splice=False, max_intron_len=None, spliced_alignment=False):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
@@ -149,16 +163,14 @@ class Mapper:
             raise ValueError(f"mid_occ_frac must be in [0, 1), not {mid_occ_frac!r}")
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand,
-                                        splice=splice, max_intron_len=max_intron_len)
+                                        splice=splice, max_intron_len=max_intron_len, spliced_alignment=spliced_alignment)
         if hpc:
             self.io.flag |= I_HPC
         if mid_occ_frac is not None:
             self.mo.mid_occ_frac = mid_occ_frac
         if split:
             self.mo.split_prefix = b"split"  # any prefix: the merge runs in memory and writes no file
-            rc = self.L.wm_check_opt(C.byref(self.io), C.byref(self.mo))
-            if rc < 0:
-                raise ValueError(f"mm_check_opt-style validation failed: {rc}")
+            _check(self.L, self.io, self.mo, spliced_alignment)
         self.n_threads = n_threads or max(1, min(64, (os.cpu_count() or 2) // 2))
         if blob is not None:  # index received from another rank (numpy uint8 array)
             self._blob_keep = blob
