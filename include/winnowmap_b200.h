@@ -97,6 +97,11 @@ int wm_sketch_batch(const wm_bloom_t *bloom, int n, const char *seq, const int64
 int wm_sketch_batch_hpc(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, const uint32_t *rid,
                         int w, int k, wm128_t **out, int64_t **out_off);
 
+/* Batched sdust_core (src/sdust.c:134): the low-complexity regions that -T masks, threshold T (1..2^20) and window W
+ * (3..64; the mapper uses 64).  seq / off as for wm_sketch_batch.  Output: the regions of sequence i, start << 32 | end, sorted
+ * and disjoint, at reg[reg_off[i] .. reg_off[i+1]); *reg / *reg_off are malloc()ed by the callee and owned by the caller. */
+int wm_sdust_batch(int n, const char *seq, const int64_t *off, int T, int W, uint64_t **reg, int64_t **reg_off);
+
 /* radix_sort_128x (src/misc.c:156; src/ksort.h:116-151) on n_arr independent arrays:
  * array i is a[off[i] .. off[i+1]); sorted in place with the reference's tie order. */
 int wm_radix_sort_128x_batch(int n_arr, wm128_t *a, const int64_t *off);
@@ -392,7 +397,10 @@ void wm_prof_get(double *out13);
 void wm_prof_get_copies(double *out2);
 /* the sketch stage alone (wm_sketch_batch without the copies out), plain or with is_hpc; *ms = mean CUDA-event time of
  * one call over `reps` calls on reads already packed on the device (tools/bench_hpc.py) */
-int wm_bench_sketch(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, int w, int k, int is_hpc, int reps, double *ms); /* bytes copied host-to-device / device-to-host by the mapping path since wm_prof_reset */
+int wm_bench_sketch(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, int w, int k, int is_hpc, int reps, double *ms);
+/* the SDUST kernel alone (wm_sdust_batch without the copies, W = 64); *ms = mean CUDA-event time of one run over `reps` runs
+ * (tools/bench_sdust.py) */
+int wm_bench_sdust(int n, const char *seq, const int64_t *off, int T, int reps, double *ms); /* bytes copied host-to-device / device-to-host by the mapping path since wm_prof_reset */
 int wm_device_synchronize(void);
 int wm_device_mem(double *free_bytes, double *total_bytes); /* cudaMemGetInfo of the current device */
 void wm_dump_timers(void); /* prints and resets the orchestration wall-clock accumulators (stderr) */

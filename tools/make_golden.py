@@ -843,8 +843,65 @@ def main_cli():
     json.dump(manifest, open(os.path.join(gdir, "cli_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- SDUST (-T): tests/golden/sdust_manifest.json and sdust_*; the other manifests are not touched ----
+# Inputs with microsatellites and tandem arrays: "tandem" is the ont_tandem case (mapped, or overlapped with itself for -X),
+# "tx" the spliced read set of the splice_* cases.  Every case must differ from the same command without -T.
+SDUST_CASES = {
+    # name: (inputs, reference options, library options of Mapper)
+    "sdust_tandem_T10": ("tandem", ["-x", "map-ont", "-c", "-T", "10"], dict(preset="map-ont", sdust_thres=10)),
+    "sdust_tandem_T20": ("tandem", ["-x", "map-ont", "-c", "-T", "20"], dict(preset="map-ont", sdust_thres=20)),
+    "sdust_tandem_a": ("tandem", ["-x", "map-ont", "-a", "-T", "20"], dict(preset="map-ont", sam=True, sdust_thres=20)),
+    "sdust_tandem_H": ("tandem", ["-x", "map-ont", "-H", "-c", "-T", "10"], dict(preset="map-ont", hpc=True, sdust_thres=10)),
+    "sdust_tandem_I_split": ("tandem", ["-x", "map-ont", "-c", "-I", "199999", "--split-prefix", "SPLIT", "-T", "20"],
+                             dict(preset="map-ont", part_bases=199999, split=True, sdust_thres=20)),
+    "sdust_tandem_X": ("tandem_ava", ["-x", "map-ont", "-X", "-T", "20"], dict(preset="map-ont", cigar=False, all_vs_all=True, sdust_thres=20)),
+    "sdust_splice": ("tx", ["-x", "splice", "-T", "20"], dict(preset="splice", cigar=False, sdust_thres=20)),
+    "sdust_tx_ont_c": ("tx", ["-x", "map-ont", "-c", "-T", "20"], dict(preset="map-ont", sdust_thres=20)),
+}
+
+
+def make_sdust_inputs(inputs, outdir):
+    """(index FASTA, reads FASTA, -W file or None) of one SDUST input set."""
+    if inputs == "tx":
+        return make_splice_inputs("tx", outdir)
+    ref, reads, wfile = make_inputs("ont_tandem", outdir)
+    return (reads, reads, None) if inputs == "tandem_ava" else (ref, reads, wfile)
+
+
+def main_sdust():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_sdust"
+    manifest = {}
+    for name, (inputs, args, lib_opts) in SDUST_CASES.items():
+        ref, reads, wfile = make_sdust_inputs(inputs, tmp)
+        outs = []
+        for a in (args, args[:args.index("-T")] + args[args.index("-T") + 2:]):
+            a = [x if x != "SPLIT" else os.path.join(tmp, name + ".split") for x in a]
+            cmd = [refbin, "-t", "4"] + a + (["-W", wfile] if wfile else []) + [ref, reads]
+            outs.append(subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout)
+        sam = "-a" in args
+        out, out0 = (sam_without_pg(o) if sam else o for o in outs)
+        assert out != out0, f"{name}: -T changes nothing"
+        with gzip.GzipFile(os.path.join(gdir, name + (".sam.stripped.gz" if sam else ".paf.gz")), "wb", mtime=0) as f:
+            f.write(sam_strip_seq(out) if sam else out)
+        manifest[name] = dict(inputs=inputs, lib=lib_opts, sam=sam, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile) if wfile else None,
+                              # not "cmd": the command-line parse check replays every "cmd" of the manifests, and the command line
+                              # refuses -T
+                              ref_cmd=" ".join(["winnowmap"] + [x if x != "SPLIT" else "<prefix>" for x in args] +
+                                               (["-W", "rep.txt"] if wfile else []) + ["ref.fa", "reads.fa"]),
+                              out_md5=hashlib.md5(out).hexdigest(), n_lines=out.count(b"\n"),
+                              n_lines_differing=len(set(out.split(b"\n")) ^ set(out0.split(b"\n"))))
+        print(name, manifest[name]["n_lines"], "lines,", manifest[name]["n_lines_differing"], "differ from the run without -T")
+    json.dump(manifest, open(os.path.join(gdir, "sdust_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
-    if "--cli" in sys.argv:
+    if "--sdust" in sys.argv:
+        main_sdust()
+    elif "--cli" in sys.argv:
         main_cli()
     elif "--splice-aln" in sys.argv:
         main_splice_aln()

@@ -22,6 +22,7 @@ using namespace wmh;
 
 static_assert(WM_SKIP_NO_DIAG == SKIP_NO_DIAG && WM_SKIP_NO_DUAL == SKIP_NO_DUAL && WM_SKIP_FOR_ONLY == SKIP_FOR_ONLY &&
               WM_SKIP_REV_ONLY == SKIP_REV_ONLY && WM_SKIP_NAME_EQ == SKIP_NAME_EQ, "seed filter bits");
+static_assert(WM_SDUST_MAX_T == SDUST_MAX_T, "-T range");
 
 // ---- small data-movement kernels ----
 // Masked copy of a window (src/map.c:795-801: covered bases become ambiguous) as a packed sequence of its own: one thread
@@ -97,6 +98,7 @@ struct GpuBackendImpl {
 	char *h_stage = 0; size_t h_stage_cap = 0; // pinned staging buffer of begin_batch
 	// workspaces
 	wm_sketch_ws sk; wm_seed_ws sd, sd2; wm_chain_ws ch; wm_extd2_ws dpws;
+	int sdust_T = 0; wm_sdust_ws sdw; // -T (0: off; sdw is then never touched)
 	wm_dbuf masked_pk, masked_nm, mask_tasks, mask_toff, mask_pool, qlen_buf, skip_buf, pre_buf, cat_tasks, cat_toff, cat_a, set_id, off_buf, nb_off, nu_off, b_out, u_out;
 	wm_dbuf nc_buf, scan_tmp, coop_ids, g_jobs, g_joff, seq_pool, dp_jobs, bt, ez, cig, cig_off, cig_out, ll_jobs, ll_scr, ll_out, mat;
 	// host result pools
@@ -133,6 +135,7 @@ public:
 	}
 	void begin_batch(const std::vector<const wm_read*> &reads) override;
 	void set_resident_pool(const char *device_ascii) override { g.resident_pool = device_ascii; }
+	bool set_sdust(int T) override { g.sdust_T = T > 0 ? T : 0; return true; }
 	void seed_chain(const std::vector<SeedTask> &tasks, const int32_t *mask_pool, const wm_pair_t *pre_pool, const ChainParams cp[2], int max_occ, std::vector<SeedOut> &out) override;
 	void run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin> &wins, const DpScoring &sc, std::vector<DpRes> &res) override;
 	void run_ll(const std::vector<LlJob> &jobs, const std::vector<MapWin> &wins, const DpScoring &sc, std::vector<LlRes> &res) override;
@@ -253,9 +256,15 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 		if (ns == 0) continue;
 		int64_t n_mz = 0;
 		{
+			wm_dust_view dv, *dust = 0;
+			if (g.sdust_T > 0) { // the regions of the sequences this pass sketches (stage-1 windows, masked copies or whole reads)
+				WM_TIMED("seed.sdust");
+				wm_sdust_run(&g.sdw, pass == 0 ? rd : rd_masked, skt.data(), ns, g.sdust_T, 64, &dv, st);
+				dust = &dv;
+			}
 			WM_TIMED("seed.sketch");
-			if (hpc) wm_sketch_run_hpc(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st);
-			else wm_sketch_run(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st);
+			if (hpc) wm_sketch_run_hpc(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st, dust);
+			else wm_sketch_run(&g.sk, g.bf, pass == 0 ? rd : rd_masked, skt.data(), ns, w, k, &n_mz, st, dust);
 		}
 		WM_TIMED("seed.lookup_sort");
 		std::vector<int32_t> qlen(ns);
@@ -286,6 +295,7 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 			WM_CUDA_CHECK(wm_memcpy_async(pass_mzspan[pass].data(), d_sp, n_mz, cudaMemcpyDeviceToHost, st));
 		}
 		wm_stream_sync(st);
+		if (g.sdust_T > 0) wm_sdust_check(&g.sdw);
 		for (int i = 0; i < ns; ++i) {
 			const int t = ids[i];
 			g.h_rep[t] = rep[i];

@@ -15,6 +15,7 @@ namespace wmh {
 struct MapWin { int32_t read, wb, wl; }; // a query window: bases [wb, wb+wl) of read `read`
 
 enum { SEED_MASKED = 1, SEED_NO_SKETCH = 2 };
+enum { SDUST_MAX_T = 1 << 20 }; // the largest -T taken (sdust.cuh: WM_SDUST_MAX_T)
 
 // The per-occurrence filter of skip_seed (src/map.c:132-154) as integer tests.  SKIP_NO_DIAG / SKIP_NO_DUAL are set only
 // when the read has a name; with the index names in strcmp order (wm_host_idx::name_rank), for the occurrence's rid:
@@ -63,6 +64,9 @@ public:
 	virtual ~Backend() {}
 	virtual void begin_batch(const std::vector<const wm_read*> &reads) = 0;
 	virtual void set_resident_pool(const char *device_ascii) { (void)device_ascii; } // reads with dev_off >= 0 are taken from here instead of the host
+	// -T: the SDUST threshold of the next seed_chain calls (0: off).  Returns whether the backend applies it; one that cannot
+	// keeps the default, and map_batch refuses T > 0 on it instead of mapping as if T were 0.
+	virtual bool set_sdust(int T) { (void)T; return false; }
 	virtual void seed_chain(const std::vector<SeedTask> &tasks, const int32_t *mask_pool, const wm_pair_t *pre_pool,
 	                        const ChainParams cp[2], int max_occ, std::vector<SeedOut> &out) = 0;
 	// `wins[job.task]` locates the query window of each job

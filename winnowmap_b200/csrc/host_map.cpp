@@ -175,6 +175,15 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		fprintf(stderr, "[ERROR] winnowmap-b200: mid_occ_frac (-f) reached the batch unresolved: set mid_occ from the index first (wm_mapopt_update)\n");
 		exit(1);
 	}
+	// -T: SDUST on every sequence sketched (src/map.c:80-81), in the three stages alike (their option sets copy sdust_thres)
+	if (opt->sdust_thres > SDUST_MAX_T) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: sdust_thres (-T) must be at most %d\n", (int)SDUST_MAX_T);
+		exit(1);
+	}
+	if (!be->set_sdust(opt->sdust_thres > 0 ? opt->sdust_thres : 0) && opt->sdust_thres > 0) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: this backend does not apply sdust_thres (-T) above 0\n");
+		exit(1);
+	}
 	const double t_batch0 = Timers::now();
 	be->begin_batch(reads);
 	g_timers.add("batch.begin_upload", Timers::now() - t_batch0);

@@ -262,6 +262,35 @@ __global__ void wm_sketch_count_kernel(const wm_sk_task *__restrict__ tasks, con
 	cnt[ch] = n;
 }
 
+// -T: clears the flag of every minimizer mm_dust_minier (src/map.c:43-67) squeezes out, so that the count and emit passes never
+// see it.  HPC: positions and spans as the emit pass makes them.
+template <bool HPC>
+__global__ void wm_sketch_dust_kernel(const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ chunk_off, const int64_t *__restrict__ base_off,
+                                      int n_tasks, int64_t n_chunks, int k, const wm_dust_view dv, uint8_t *__restrict__ flag_all,
+                                      const int32_t *__restrict__ pos)
+{
+	const int64_t ch = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (ch >= n_chunks) return;
+	int lo = 0, hi = n_tasks;
+	while (hi - lo > 1) { int m = (lo + hi) >> 1; if (chunk_off[m] <= ch) lo = m; else hi = m; }
+	const int n_reg = dv.reg_n[lo];
+	if (n_reg == 0) return;
+	const wm_sk_task T = tasks[lo];
+	const uint64_t *reg = dv.reg + dv.reg_off[lo];
+	uint8_t *flag = flag_all + base_off[lo];
+	const int c0 = (int)(ch - chunk_off[lo]) * WM_SK_CH;
+	int c1 = c0 + WM_SK_CH; if (c1 > T.len) c1 = T.len;
+	for (int i = c0; i < c1; ++i)
+		if (flag[i]) {
+			int32_t p = i, span = k;
+			if (HPC) {
+				const int64_t q = T.seq_off + i;
+				p = pos[q], span = pos[q] - (i >= k ? pos[q - k] : -1);
+			}
+			if (!wm_dust_keep(reg, n_reg, p, span)) flag[i] = 0;
+		}
+}
+
 // HPC: positions and spans come from the symbol -> base map
 template <bool HPC>
 __global__ void wm_sketch_emit_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, const int64_t *__restrict__ chunk_off,
@@ -398,7 +427,7 @@ void wm_pack_gather(const char *d_pool, const int64_t *d_src_off, const int64_t 
 // `pos` its symbol -> base map (wm_sketch_run_hpc).
 template <bool HPC>
 static void wm_sketch_passes(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                             int w, int k, const int32_t *pos, int64_t *n_mz, cudaStream_t st)
+                             int w, int k, const int32_t *pos, int64_t *n_mz, cudaStream_t st, const wm_dust_view *dust)
 {
 	*n_mz = 0;
 	std::vector<int64_t> h_off(3 * (size_t)(n_tasks + 1));
@@ -433,6 +462,11 @@ static void wm_sketch_passes(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_
 		wm_count_launch(); wm_sketch_seq_kernel<HPC><<<(n_tasks + 63) / 64, 64, 0, st>>>(seq, d_tasks, d_base_off, n_tasks, w, k, bf, d_flag, d_ring, pos);
 		WM_CUDA_CHECK(cudaGetLastError());
 	}
+	if (dust) {
+		wm_count_launch(); wm_sketch_dust_kernel<HPC><<<(unsigned)((n_chunks + 127) / 128), 128, 0, st>>>(d_tasks, d_chunk_off, d_base_off, n_tasks, n_chunks, k,
+		                                                                                              *dust, d_flag, pos);
+		WM_CUDA_CHECK(cudaGetLastError());
+	}
 	int32_t *d_cnt = (int32_t*)ws->cnt.need(sizeof(int32_t) * (n_chunks + 1));
 	int64_t *d_rank = (int64_t*)ws->rank.need(sizeof(int64_t) * (n_chunks + 2));
 	int64_t *d_tmp = (int64_t*)ws->scan_tmp.need(sizeof(int64_t) * wm_scan_tmp_elems(n_chunks));
@@ -455,9 +489,9 @@ static void wm_sketch_passes(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_
 }
 
 void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                   int w, int k, int64_t *n_mz, cudaStream_t st)
+                   int w, int k, int64_t *n_mz, cudaStream_t st, const wm_dust_view *dust)
 {
-	wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st);
+	wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st, dust);
 }
 
 // ---- homopolymer-compressed sketch: a compaction front end, then the passes above on the compressed slices ----
@@ -526,13 +560,13 @@ wm_hpc_pack_kernel(const wm_pkseq seq, const wm_sk_task *__restrict__ tasks, con
 }
 
 void wm_sketch_run_hpc(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                       int w, int k, int64_t *n_mz, cudaStream_t st)
+                       int w, int k, int64_t *n_mz, cudaStream_t st, const wm_dust_view *dust)
 {
 	*n_mz = 0;
 	std::vector<int64_t> grp_off(n_tasks + 1, 0);
 	for (int i = 0; i < n_tasks; ++i) grp_off[i + 1] = grp_off[i] + (h_tasks[i].len > 0 ? (h_tasks[i].len + 31) / 32 : 0);
 	const int64_t n_groups = grp_off[n_tasks];
-	if (n_tasks == 0 || n_groups == 0) { wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st); return; }
+	if (n_tasks == 0 || n_groups == 0) { wm_sketch_passes<false>(ws, bf, seq, h_tasks, n_tasks, w, k, 0, n_mz, st, dust); return; }
 	wm_sk_task *d_tasks = (wm_sk_task*)ws->hpc_tasks.need(sizeof(wm_sk_task) * n_tasks);
 	int64_t *d_goff = (int64_t*)ws->hpc_goff.need(sizeof(int64_t) * (n_tasks + 1));
 	int64_t *d_coff = (int64_t*)ws->hpc_coff.need(sizeof(int64_t) * (n_tasks + 1));
@@ -563,7 +597,7 @@ void wm_sketch_run_hpc(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq 
 	wm_stream_sync(st);
 	std::vector<wm_sk_task> ct(n_tasks);
 	for (int i = 0; i < n_tasks; ++i) ct[i].seq_off = coff[i], ct[i].len = (int32_t)(coff[i + 1] - coff[i]), ct[i].rid = h_tasks[i].rid;
-	wm_sketch_passes<true>(ws, bf, cs, ct.data(), n_tasks, w, k, d_pos, n_mz, st);
+	wm_sketch_passes<true>(ws, bf, cs, ct.data(), n_tasks, w, k, d_pos, n_mz, st, dust);
 }
 
 // one byte per minimizer: its span (x & 0xff)

@@ -1,6 +1,7 @@
 #pragma once
 #include "wm_common.cuh"
 #include "pkseq.cuh"
+#include "sdust.cuh"
 
 struct wm128_dev { uint64_t x, y; };
 
@@ -36,12 +37,27 @@ static inline size_t wm_nm_words(int64_t n) { return (size_t)((n + 31) / 32) + W
 // ASCII (16-byte aligned device buffer) -> packed pool; the second form gathers reads scattered over a device ASCII pool
 void wm_pack_ascii(const char *d_in, int64_t n, uint32_t *d_pk, uint32_t *d_nm, cudaStream_t st);
 void wm_pack_gather(const char *d_pool, const int64_t *d_src_off, const int64_t *d_dst_off, int n_reads, int64_t n, uint32_t *d_pk, uint32_t *d_nm, cudaStream_t st);
+// dust (may be null): the SDUST regions of the tasks (wm_sdust_run); a minimizer mm_dust_minier would remove is not emitted
 void wm_sketch_run(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                   int w, int k, int64_t *n_mz, cudaStream_t st);
+                   int w, int k, int64_t *n_mz, cudaStream_t st, const wm_dust_view *dust = 0);
 // the same on homopolymer-compressed sequences (mm_sketch with is_hpc = 1): the tasks are compacted on the device first;
-// positions and spans of the minimizers refer to the uncompressed bases
+// positions and spans of the minimizers refer to the uncompressed bases (and the SDUST regions to the uncompressed tasks)
 void wm_sketch_run_hpc(wm_sketch_ws *ws, const wm_bloom_dev &bf, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks,
-                       int w, int k, int64_t *n_mz, cudaStream_t st);
+                       int w, int k, int64_t *n_mz, cudaStream_t st, const wm_dust_view *dust = 0);
+// SDUST (sdust.cu) of every task with threshold T and window W (3..WM_SDUST_WMAX); *view points into ws on return
+// (asynchronous on st: wm_sdust_check after the caller's next synchronisation of st exits if the regions overflowed)
+struct wm_sdust_ws {
+	wm_dbuf tasks, order, back, reg_off, reg_n, reg, P, err;
+	int *h_err = 0; // pinned
+	void release()
+	{
+		tasks.release(); order.release(); back.release(); reg_off.release(); reg_n.release(); reg.release(); P.release(); err.release();
+		if (h_err) cudaFreeHost(h_err), h_err = 0;
+	}
+	~wm_sdust_ws() { if (h_err) cudaFreeHost(h_err); }
+};
+void wm_sdust_run(wm_sdust_ws *ws, const wm_pkseq &seq, const wm_sk_task *h_tasks, int n_tasks, int T, int W, wm_dust_view *view, cudaStream_t st);
+void wm_sdust_check(const wm_sdust_ws *ws);
 // span (x & 0xff) of each of n minimizers
 void wm_mz_spans(const wm128_dev *d_mz, int64_t n, uint8_t *d_span, cudaStream_t st);
 void wm_bloom_dev_from_table(wm_bloom_dev *d, const uint8_t *d_table, uint64_t bits);

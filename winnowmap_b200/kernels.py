@@ -144,6 +144,28 @@ def sketch_batch(bloom, seqs, w, k, rids=None, hpc=False):
     return [xy[o[i]: o[i + 1]].copy() for i in range(n)]
 
 
+def sdust_batch(seqs, T, W=64):
+    """Batched sdust_core (reference src/sdust.c:134), the regions -T masks.  seqs: list of bytes.  Returns a list of (n,2)
+    int64 arrays of [start, end) per sequence."""
+    n = len(seqs)
+    off = np.zeros(n + 1, dtype=np.int64)
+    if n:
+        off[1:] = np.cumsum([len(s) for s in seqs])
+    buf = b"".join(seqs) + b"\0"
+    reg, reg_off = C.c_void_p(), C.c_void_p()
+    L = lib()
+    L.wm_sdust_batch.argtypes = [C.c_int, C.c_char_p, i64p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    if L.wm_sdust_batch(n, buf, _p(off, i64p), T, W, C.byref(reg), C.byref(reg_off)) != 0:
+        raise ValueError(f"wm_sdust_batch failed (T = {T}, W = {W})")
+    o = np.ctypeslib.as_array(C.cast(reg_off, i64p), shape=(n + 1,)).copy()
+    tot = int(o[-1])
+    r = np.ctypeslib.as_array(C.cast(reg, u64p), shape=(max(tot, 1),)).copy()[:tot]
+    _libc.free(reg)
+    _libc.free(reg_off)
+    se = np.stack([(r >> np.uint64(32)).astype(np.int64), (r & np.uint64(0xffffffff)).astype(np.int64)], axis=1)
+    return [se[o[i]: o[i + 1]].copy() for i in range(n)]
+
+
 def radix_sort_128x_batch(arrays):
     """radix_sort_128x (reference src/misc.c:156) on each (n,2) uint64 array, tie order included."""
     n = len(arrays)

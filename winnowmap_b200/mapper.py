@@ -32,6 +32,7 @@ F_CIGAR, F_OUT_SAM, F_OUT_CG, F_NO_PRINT_2ND, F_PAF_NO_HIT = 0x004, 0x008, 0x020
 F_NO_DIAG, F_NO_DUAL, F_NO_LJOIN, F_FOR_ONLY, F_REV_ONLY, F_ALL_CHAINS = 0x001, 0x002, 0x400, 0x100000, 0x200000, 0x800000
 F_SPLICE, F_SPLICE_FOR, F_SPLICE_REV, F_SPLICE_FLANK = 0x080, 0x100, 0x200, 0x40000
 I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
+SDUST_MAX_T = 1 << 20  # the largest -T the library takes (csrc/sdust.cuh)
 
 STAT_NAMES = ("n_reads", "n_bases", "n_minimaps", "n_chained", "n_dp_jobs", "n_ll_jobs", "n_rounds", "t_seed", "t_dp", "t_host",
               "t_index", "t_map", "n_keys", "n_pos", "n_topfreq", "topfreq_threshold", "t_topfreq")
@@ -148,11 +149,13 @@ class Mapper:
     preset="splice" / "splice:hq" / "cdna" with cigar=False maps spliced reads (approximate PAF, cDNA chaining); splice=True is
     --splice and max_intron_len is -G (make_options).  With spliced_alignment=True they also align at base level (-c, or -a
     with sam=True): ksw_exts2 on the GPU, both transcript strands tried per hit, ts:A, introns as N; the other flags of the
-    reference (--eqx, --cs, --MD, -u, --splice-flank, -C, --cap-sw-mem) are the fields of self.mo."""
+    reference (--eqx, --cs, --MD, -u, --splice-flank, -C, --cap-sw-mem) are the fields of self.mo.
+    sdust_thres=T is -T: minimizers that lie mostly in low-complexity regions (SDUST with threshold T, window 64) are dropped
+    before seeding, in every stage; 0 (the default) is off.  The command line still refuses -T; the library applies it."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
                  no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None,
-                 splice=False, max_intron_len=None, spliced_alignment=False):
+                 splice=False, max_intron_len=None, spliced_alignment=False, sdust_thres=0):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
@@ -161,6 +164,8 @@ class Mapper:
             raise ValueError("part_bases must be a positive number of bases and cannot be combined with blob=")
         if mid_occ_frac is not None and not 0.0 <= mid_occ_frac < 1.0:
             raise ValueError(f"mid_occ_frac must be in [0, 1), not {mid_occ_frac!r}")
+        if not 0 <= int(sdust_thres) <= SDUST_MAX_T:
+            raise ValueError(f"sdust_thres must be in 0..{SDUST_MAX_T}, not {sdust_thres!r}")
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand,
                                         splice=splice, max_intron_len=max_intron_len, spliced_alignment=spliced_alignment)
@@ -168,6 +173,7 @@ class Mapper:
             self.io.flag |= I_HPC
         if mid_occ_frac is not None:
             self.mo.mid_occ_frac = mid_occ_frac
+        self.mo.sdust_thres = int(sdust_thres)
         if split:
             self.mo.split_prefix = b"split"  # any prefix: the merge runs in memory and writes no file
             _check(self.L, self.io, self.mo, spliced_alignment)
