@@ -43,6 +43,17 @@ typedef struct {
 	int32_t reserved;
 } wm_extz_t;
 
+/* Junction intervals of an index (mm_idx_intv1_t / mm_idx_intv_t, src/index.c, what mm_idx_bed_read leaves in mm_idx_t::I):
+ * one wm_idx_intv_t per sequence, its n intervals sorted by st.  strand is 1 (+), -1 (-) or 0 (neither); max is unused. */
+typedef struct {
+	int32_t st, en, max;
+	int32_t score:30, strand:2;
+} wm_idx_intv1_t;
+typedef struct {
+	int32_t n, m;
+	wm_idx_intv1_t *a;
+} wm_idx_intv_t;
+
 /* library / device */
 const char *wm_version(void);
 int wm_device_count(void);                 /* number of visible CUDA devices (0 if none) */
@@ -102,6 +113,12 @@ int wm_sketch_batch_hpc(const wm_bloom_t *bloom, int n, const char *seq, const i
  * and disjoint, at reg[reg_off[i] .. reg_off[i+1]); *reg / *reg_off are malloc()ed by the callee and owned by the caller. */
 int wm_sdust_batch(int n, const char *seq, const int64_t *off, int T, int W, uint64_t **reg, int64_t **reg_off);
 
+/* Batched mm_idx_bed_junc (src/index.c:780-803): the junction annotation of n_win target windows, on the device.  I: n_seq
+ * records as wm_idx_bed_read / mm_idx_bed_read leave them (each sorted by st).  Window i is bases [off, off + len) of sequence
+ * rid, win[4 i .. 4 i + 3] = (rid, off, len, reversed); reversed gives the bytes in reverse order (mm_seq_rev: the bits are
+ * not swapped).  Its len bytes go to out[out_off[i] ..); a rid outside [0, n_seq) gives zeros.  0, or -1 on a bad argument. */
+int wm_bed_junc_batch(const wm_idx_intv_t *I, int n_seq, int n_win, const int32_t *win, uint8_t *out, const int64_t *out_off);
+
 /* radix_sort_128x (src/misc.c:156; src/ksort.h:116-151) on n_arr independent arrays:
  * array i is a[off[i] .. off[i+1]); sorted in place with the reference's tie order. */
 int wm_radix_sort_128x_batch(int n_arr, wm128_t *a, const int64_t *off);
@@ -142,6 +159,7 @@ typedef struct {
 	uint64_t bloom_bits;           /* bloom_filter::size() */
 	const uint8_t *bloom_table;    /* bloom_filter::table() */
 } wm_idx_view_t;
+
 
 
 /* ---- structs that cross the boundary: field-for-field the reference's public structs ---- */
@@ -256,10 +274,21 @@ wm_gpu_ctx *wm_gpu_idx_upload(const wm_idx_view_t *idx, int device);
  * sketched homopolymer-compressed and the alignment anchors are adjusted as mm_adjust_minier does (src/align.c:350-365).
  * Any other bit is refused (NULL).  wm_gpu_idx_upload(idx, device) is wm_gpu_idx_upload_flag(idx, 0, device). */
 wm_gpu_ctx *wm_gpu_idx_upload_flag(const wm_idx_view_t *idx, int idx_flag, int device);
-/* Set in idx_flag by the caller when mm_idx_t::I holds junction intervals (--junc-bed, mm_idx_bed_read).  Junction annotation
- * is not built: such a context maps, but spliced base-level alignment on it (MM_F_SPLICE | MM_F_CIGAR) is refused with a message
- * and exit(1) instead of aligning without the intervals. */
+/* Set in idx_flag by the caller when mm_idx_t::I holds junction intervals (--junc-bed, mm_idx_bed_read).  The context then
+ * needs those intervals too: hand them over with wm_idx_set_junc (or read the BED again with wm_idx_bed_read).  Until then it
+ * maps, but spliced base-level alignment on it (MM_F_SPLICE | MM_F_CIGAR) is refused with a message and exit(1) instead of
+ * aligning without the intervals. */
 #define WM_IDX_JUNC 0x100
+/* mm_idx_bed_read(mi, fn, 1) (src/index.c:769-778; src/main.c:416): the junction intervals of a BED file (plain or gzip, "-"
+ * for stdin) for the sequences of the context, per part of a multi-part index with that part's names as the reference reads it
+ * once per part.  BED12 lines give their introns (the gaps between consecutive blocks), other lines [start, end) itself.  They
+ * replace any intervals set before and go to the device, where every DP of spliced base-level alignment gets the annotation
+ * of its target window (mm_idx_bed_junc, src/align.c:688-794), which adds junc_bonus at annotated donors and acceptors.  Other
+ * mapping is unchanged.  0, or -1 when the file cannot be opened. */
+int wm_idx_bed_read(wm_gpu_ctx *ctx, const char *fn);
+/* The same from intervals already read: I is the reference's mm_idx_t::I after mm_idx_bed_read (wm_idx_n_seq(ctx) records in
+ * that layout, each sorted by st), for a context of a single index or one part.  0, or -1 on a multi-part root. */
+int wm_idx_set_junc(wm_gpu_ctx *ctx, const wm_idx_intv_t *I);
 /* the index flag the context maps with (MM_I_HPC or 0) */
 int wm_idx_flag(const wm_gpu_ctx *ctx);
 void wm_gpu_destroy(wm_gpu_ctx *ctx);
@@ -332,7 +361,8 @@ wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
  * device.  Its name tests compare names[i] with the index's sequence names; names == NULL or names[i] == NULL is a read
  * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE maps with the cDNA chaining of the reference;
  * with MM_F_CIGAR it also aligns as mm_align_skeleton does for splice (ksw_exts2 on the device, both transcript strands per hit
- * under MM_F_SPLICE_FOR | MM_F_SPLICE_REV, ts:A), without junction annotation.  MM_F_SR and MM_F_HEAP_SORT are refused. */
+ * under MM_F_SPLICE_FOR | MM_F_SPLICE_REV, ts:A), with the junction annotation of wm_idx_bed_read / wm_idx_set_junc when the
+ * context has intervals.  MM_F_SR and MM_F_HEAP_SORT are refused. */
 int wm_gpu_map_batch(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, int n_seq, const char *const *names, const char *const *seqs,
                      const int32_t *lens, int32_t *n_reg, wm_reg1_t **reg, int32_t *rep_len, int32_t *frag_gap, int n_threads);
 
@@ -395,6 +425,9 @@ void wm_prof_reset(void);
  * bytes (SURVEY.md 8d), units (block cells / anchors), DP jobs */
 void wm_prof_get(double *out13);
 void wm_prof_get_copies(double *out2);
+/* junction annotation of the mapping path since the last call with reset != 0: out[0] launches of the annotation kernel, out[1]
+ * target windows annotated, out[2] the kernel's CUDA-event milliseconds (counted while wm_prof_enable is on) */
+void wm_junc_stats(double *out3, int reset);
 /* the sketch stage alone (wm_sketch_batch without the copies out), plain or with is_hpc; *ms = mean CUDA-event time of
  * one call over `reps` calls on reads already packed on the device (tools/bench_hpc.py) */
 int wm_bench_sketch(const wm_bloom_t *bloom, int n, const char *seq, const int64_t *off, int w, int k, int is_hpc, int reps, double *ms);

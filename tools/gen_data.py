@@ -137,13 +137,15 @@ def _revcomp(seq):
     return COMP[seq[::-1]]
 
 
-def make_transcriptome(rng, genome_len, n_genes, n_contigs=2, long_introns=2, long_genes=3, n_paralogs=3):
+def make_transcriptome(rng, genome_len, n_genes, n_contigs=2, long_introns=2, long_genes=3, n_paralogs=3, layout=None):
     """A seeded spliced-transcript setting: (contigs, transcripts).  contigs: i.i.d. genome sequence with multi-exon genes on
     both strands.  Introns are GT-AG on the plus strand and CT-AC (their reverse complement) on the minus strand, except about
     one in twenty, which keeps random donor / acceptor bases; their lengths are log-uniform from 60 bp to 20 kb, plus
     `long_introns` introns above 200 kb.  The first `long_genes` genes have a long last exon, so that their transcripts exceed
     10 kb.  Every gene of three or more exons also gets an isoform that skips one internal exon, and `n_paralogs` genes get a
-    copy elsewhere (exons 3 % divergent, introns of their own).  transcripts: (name, mRNA as uint8 in the gene's sense, 5' to 3')."""
+    copy elsewhere (exons 3 % divergent, introns of their own).  transcripts: (name, mRNA as uint8 in the gene's sense, 5' to 3').
+    layout, when a list, gets one (name, contig name, strand, [(start, end) of each exon on the contig, ascending]) per
+    transcript, in the order of `transcripts` (the random draws are the same either way)."""
     contigs = [random_seq(rng, genome_len // n_contigs) for _ in range(n_contigs)]
     cursor = [1000] * n_contigs
     exon_seqs, transcripts, n_long = [], [], 0
@@ -163,10 +165,11 @@ def make_transcriptome(rng, genome_len, n_genes, n_contigs=2, long_introns=2, lo
         if start + span + 1000 > len(seq):
             return None
         cursor[ci] = start + span
-        pos, parts = start, []
+        pos, parts, coords = start, [], []
         for e, body in enumerate(bodies):
             seq[pos:pos + len(body)] = body
             parts.append(body)
+            coords.append((pos, pos + len(body)))
             pos += len(body)
             if e < len(introns):
                 end = pos + introns[e]
@@ -174,13 +177,15 @@ def make_transcriptome(rng, genome_len, n_genes, n_contigs=2, long_introns=2, lo
                     seq[pos:pos + 2] = np.frombuffer(b"GT" if strand == "+" else b"CT", np.uint8)
                     seq[end - 2:end] = np.frombuffer(b"AG" if strand == "+" else b"AC", np.uint8)
                 pos = end
-        isoforms = [parts]
+        isoforms = [(parts, coords)]
         if len(parts) >= 3:
             skip = int(rng.integers(1, len(parts) - 1))
-            isoforms.append(parts[:skip] + parts[skip + 1:])
-        for iso, ps in enumerate(isoforms):
+            isoforms.append((parts[:skip] + parts[skip + 1:], coords[:skip] + coords[skip + 1:]))
+        for iso, (ps, cs) in enumerate(isoforms):
             m = np.concatenate(ps)
             transcripts.append((f"{name}.{iso}{strand}", m if strand == "+" else _revcomp(m)))
+            if layout is not None:
+                layout.append((transcripts[-1][0], f"chr{ci + 1}", strand, cs))
         return parts
 
     for g in range(n_genes):

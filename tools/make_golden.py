@@ -898,8 +898,148 @@ def main_sdust():
     json.dump(manifest, open(os.path.join(gdir, "sdust_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- junction annotation (--junc-bed with spliced base-level alignment): tests/golden/splice_junc_manifest.json and splice_junc_*;
+# the other manifests are not touched.  The inputs are those of the splice_aln_* cases plus a BED of the transcriptome: "full" lists
+# every transcript (isoforms and paralogs included) as BED12 with the gene's strand, "mixed" (gzipped) half of them as BED12 and
+# the other lines a reader has to drop or cut short.  Every case must differ from the same command without --junc-bed.
+JUNC_BED_SEED = 3051
+SPLICE_JUNC_CASES = {
+    # name: (reads, BED, reference options, library options)
+    "splice_junc_c": ("tx", "full", ["-x", "splice", "-c"], dict(preset="splice")),
+    "splice_junc_a": ("tx", "full", ["-x", "splice", "-a"], dict(preset="splice", sam=True)),
+    "splice_junc_hq_cs": ("tx_hq", "full", ["-x", "splice:hq", "-c", "--cs"], dict(preset="splice:hq", set_flags=F_OUT_CS)),
+    "splice_junc_cdna_md": ("tx", "full", ["-x", "cdna", "-a", "--MD"], dict(preset="cdna", sam=True, set_flags=F_OUT_MD)),
+    "splice_junc_uf": ("tx", "full", ["-x", "splice", "-c", "-u", "f"], dict(preset="splice", set_flags=F_SPLICE_FOR, clear_flags=F_SPLICE_REV)),
+    "splice_junc_ur": ("tx", "full", ["-x", "splice", "-c", "-u", "r"], dict(preset="splice", set_flags=F_SPLICE_REV, clear_flags=F_SPLICE_FOR)),
+    "splice_junc_mixed": ("tx", "mixed", ["-x", "splice", "-c"], dict(preset="splice")),
+    "splice_junc_H": ("tx", "full", ["-x", "splice", "-c", "-H"], dict(preset="splice", hpc=True)),
+    "splice_junc_I_split": ("tx", "full", ["-x", "splice", "-c", "-I", "500k", "--split-prefix", "SPLIT"],
+                            dict(preset="splice", part_bases=500000, split=True)),
+}
+
+
+def _bed12(name, chrom, strand, exons, score):
+    st, en = exons[0][0], exons[-1][1]
+    return "\t".join([chrom, str(st), str(en), name, str(score), strand, str(st), str(en), "0", str(len(exons)),
+                      ",".join(str(b - a) for a, b in exons) + ",", ",".join(str(a - st) for a, _ in exons) + ","])
+
+
+def make_junc_beds(outdir):
+    """(full BED, mixed BED.gz) of the splice transcriptome."""
+    c = SPLICE
+    layout = []
+    contigs, _ = gen_data.make_transcriptome(np.random.default_rng(c["ref_seed"]), c["genome_len"], c["n_genes"], layout=layout)
+    rng = np.random.default_rng(JUNC_BED_SEED)
+    full = [_bed12(n, ch, sd, ex, int(rng.integers(0, 1001))) for n, ch, sd, ex in layout]
+    mixed = ["track name=junctions description=\"test\"", "# introns of half the transcripts"]
+    flip = {"+": "-", "-": "+"}
+    for i, (n, ch, sd, ex) in enumerate(layout):
+        sc = int(rng.integers(0, 1001))
+        if i % 2 == 0:
+            mixed.append(_bed12(n, ch, sd, ex, sc))
+            continue
+        introns = [(ex[j][1], ex[j + 1][0]) for j in range(len(ex) - 1)]
+        for j, (a, b) in enumerate(introns):
+            kind = int(rng.integers(0, 6))
+            if kind <= 2:  # BED6, the right strand
+                mixed.append(f"{ch}\t{a}\t{b}\t{n}.i{j}\t{sc}\t{sd}")
+            elif kind == 3:  # no strand
+                mixed.append(f"{ch}\t{a}\t{b}\t{n}.i{j}\t{sc}\t.")
+            elif kind == 4:  # the wrong strand
+                mixed.append(f"{ch}\t{a}\t{b}\t{n}.i{j}\t{sc}\t{flip[sd]}")
+            else:  # BED4: no score, no strand
+                mixed.append(f"{ch}\t{a}\t{b}\t{n}.i{j}")
+    n, ch, sd, ex = layout[1]
+    b12 = _bed12(n, ch, sd, ex, 7).split("\t")
+    L = len(contigs[0][1])
+    mixed += [
+        f"chrUn\t{ex[0][1]}\t{ex[1][0]}\tunknown\t0\t+",                       # a contig the index does not have
+        f"{ch}\t{ex[0][1]}\t{ex[0][1]}\tempty\t0\t{sd}",                         # st == en
+        f"{ch}\t{ex[1][0]}\t{ex[0][1]}\treversed\t0\t{sd}",                      # st > en
+        f"{ch}\t-10\t{ex[0][1]}\tnegative\t0\t{sd}",                             # a negative start
+        "\t".join(b12[:11]),                                                     # 11 columns: [chromStart, chromEnd) itself
+        "\t".join(b12[:9] + ["x" + b12[9]] + b12[10:]),                           # a non-digit block count: the same
+        "\t".join(b12[:3] + ["crlf", "0", sd]) + "\r",                            # CRLF line ending
+        f"chr1\t{L - 300}\t{L - 100}\tnear_end\t0\t+",
+    ]
+    os.makedirs(outdir, exist_ok=True)
+    fb, mb = os.path.join(outdir, "junc_full.bed"), os.path.join(outdir, "junc_mixed.bed.gz")
+    with open(fb, "w") as f:
+        f.write("\n".join(full) + "\n")
+    with gzip.GzipFile(mb, "wb", mtime=0) as f:
+        f.write(("\n".join(mixed) + "\n").encode())
+    return fb, mb
+
+
+def make_junc_inputs(name, outdir):
+    """(genome FASTA, reads FASTA, -W file, BED) of one splice_junc_* case."""
+    reads_kind, bed = SPLICE_JUNC_CASES[name][:2]
+    ref, reads, wfile = make_splice_inputs(reads_kind, outdir)
+    fb, mb = make_junc_beds(outdir)
+    return ref, reads, wfile, fb if bed == "full" else mb
+
+
+def main_junc():
+    # the reference with the one patch its BED reader needs to read a line at all (oracle/build_junc.sh)
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap_junc")
+    if not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "winnowmap")):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    subprocess.check_call([os.path.join(ROOT, "oracle", "build_junc.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_junc"
+    manifest = {}
+    for name, (reads_kind, bed_kind, args, lib_opts) in SPLICE_JUNC_CASES.items():
+        ref, reads, wfile, bed = make_junc_inputs(name, tmp)
+        args = [a if a != "SPLIT" else os.path.join(tmp, name + ".split") for a in args]
+        outs = []
+        for extra in (["--junc-bed", bed], []):
+            cmd = [refbin, "-t", "4"] + args + extra + ["-W", wfile, ref, reads]
+            outs.append(subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout)
+        sam = "-a" in args
+        out, out0 = (sam_without_pg(o) if sam else o for o in outs)
+        n_diff = len(set(out.split(b"\n")) ^ set(out0.split(b"\n")))
+        assert n_diff > 0, f"{name}: --junc-bed changes nothing"
+        with gzip.GzipFile(os.path.join(gdir, name + (".sam.stripped.gz" if sam else ".paf.gz")), "wb", mtime=0) as f:
+            f.write(sam_strip_seq(out) if sam else out)
+        manifest[name] = dict(reads=reads_kind, bed=bed_kind, lib=lib_opts, sam=sam, ref_md5=md5(ref), reads_md5=md5(reads), w_md5=md5(wfile),
+                              bed_md5=md5(bed),
+                              # not "cmd": the command-line parse check replays every "cmd" of the manifests, and the command line
+                              # refuses spliced alignment
+                              ref_cmd=" ".join(["winnowmap"] + [a if not a.startswith(tmp) else "<prefix>" for a in args] +
+                                               ["--junc-bed", os.path.basename(bed), "-W", "rep.txt", "ref.fa", "reads.fa"]),
+                              out_md5=hashlib.md5(out).hexdigest(), n_lines=out.count(b"\n"), n_lines_differing=n_diff)
+        print(name, manifest[name]["n_lines"], "lines,", n_diff, "differ from the run without --junc-bed")
+    json.dump(manifest, open(os.path.join(gdir, "splice_junc_manifest.json"), "w"), indent=1, sort_keys=True)
+    record_junc_intervals(tmp, gdir)
+
+
+def record_junc_intervals(tmp, gdir):
+    """tests/golden/splice_junc_ref_intervals.npz: the reference's mm_idx_t::I after mm_idx_bed_read of both BEDs on the splice
+    genome's names, as raw 16-byte records (<bed>_recs) with per-contig offsets (<bed>_off)."""
+    import ctypes as C
+    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libref_harness_junc.so"))
+    names = [nm for nm, _ in read_fasta(make_splice_inputs("tx", tmp)[0])]
+    arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
+    out = {}
+    for kind, bed in zip(("full", "mixed"), make_junc_beds(tmp)):
+        assert L.ref_bed_read(len(names), arr, bed.encode()) == 0
+        recs, off = [], [0]
+        for rid in range(len(names)):
+            n = L.ref_bed_intervals(rid, None, 0)
+            buf = np.zeros(4 * n, np.int32)
+            L.ref_bed_intervals(rid, buf.ctypes.data_as(C.c_void_p), n)
+            recs.append(buf)
+            off.append(off[-1] + n)
+        out[kind + "_recs"] = np.concatenate(recs).reshape(-1, 4) if recs else np.zeros((0, 4), np.int32)
+        out[kind + "_off"] = np.array(off, np.int64)
+        out[kind + "_md5"] = np.array(md5(bed))
+    np.savez_compressed(os.path.join(gdir, "splice_junc_ref_intervals.npz"), names=np.array(names), **out)
+
+
 if __name__ == "__main__":
-    if "--sdust" in sys.argv:
+    if "--junc" in sys.argv:
+        main_junc()
+    elif "--sdust" in sys.argv:
         main_sdust()
     elif "--cli" in sys.argv:
         main_cli()

@@ -693,6 +693,23 @@ extern "C" int wm_idx_name2id(const wm_gpu_ctx_s *c, const char *name)
 	for (size_t i = 0; i < c->hidx.name.size(); ++i) if (c->hidx.name[i] == name) return (int)i;
 	return -1;
 }
+// mm_idx_bed_read(mi, fn, 1) once per index part (src/main.c:416 runs it on every part the index reader returns), each part
+// with its own names; then the intervals go to that part's device index
+extern "C" int wm_idx_bed_read(wm_gpu_ctx_s *c, const char *fn)
+{
+	for (wm_gpu_ctx_s *p : parts_of(c)) {
+		if (read_bed_junc(&p->hidx, fn) < 0) return -1;
+		gpu_backend_set_junc(p->be, &p->hidx);
+	}
+	return 0;
+}
+extern "C" int wm_idx_set_junc(wm_gpu_ctx_s *c, const wm_idx_intv_t *I)
+{
+	if (is_multi(c)) { fprintf(stderr, "[ERROR] wm_idx_set_junc: a multi-part index takes the intervals of each part (wm_idx_part)\n"); return -1; }
+	set_junc(&c->hidx, I);
+	gpu_backend_set_junc(c->be, &c->hidx);
+	return 0;
+}
 extern "C" int wm_idx_n_seq(const wm_gpu_ctx_s *c) { return (int)c->hidx.name.size(); }
 extern "C" const char *wm_idx_seq_name(const wm_gpu_ctx_s *c, int rid) { return rid >= 0 && (size_t)rid < c->hidx.name.size() ? c->hidx.name[rid].c_str() : 0; }
 extern "C" uint32_t wm_idx_seq_len(const wm_gpu_ctx_s *c, int rid) { return rid >= 0 && (size_t)rid < c->hidx.len.size() ? c->hidx.len[rid] : 0; }

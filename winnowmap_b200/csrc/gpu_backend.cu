@@ -10,6 +10,7 @@
 #include "sketch.cuh"
 #include "seed.cuh"
 #include "chain.cuh"
+#include "bed_junc.cuh"
 #include "gpu_backend.h"
 #include "host_timers.h"
 
@@ -111,6 +112,10 @@ struct GpuBackendImpl {
 	// the index this backend was created with (ix / bf / hidx above are the one it maps against, which gpu_backend_bind
 	// may point at another index of the same context: one part of a multi-part index)
 	wm_idx_dev own_ix; wm_bloom_dev own_bf; const wm_host_idx *own_hidx;
+	// junction intervals of the bound index and of the own one (n_seq 0: none; gpu_backend_set_junc), and the annotation of a
+	// splice DP launch's targets, parallel to seq_pool
+	wm_junc_dev jx = {}, own_jx = {};
+	wm_dbuf junc_pool, junc_wins;
 };
 
 class GpuBackend : public Backend {
@@ -128,6 +133,7 @@ public:
 			cudaFree((void*)x.keys); cudaFree((void*)x.pos_off); cudaFree((void*)x.pos); cudaFree((void*)x.S);
 			cudaFree((void*)x.ht_key); cudaFree((void*)x.ht_val); cudaFree((void*)g.own_bf.table);
 			cudaFree((void*)x.seq_len); cudaFree((void*)x.name_rank);
+			wm_junc_free(&g.own_jx);
 		}
 		if (g.st) cudaStreamDestroy(g.st);
 		// this thread's workspace allocations must not go on to the stream just destroyed (wm_dbuf_use_stream)
@@ -579,6 +585,20 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 			wm_count_launch(); wm_gather2_kernel<<<(unsigned)((pool_off / 16 + 255) / 256), 256, 0, st>>>(d_gj, d_joff, (int)gj.size(), rd, g.ix.S, d_pool, pool_off / 16);
 			WM_CUDA_CHECK(cudaGetLastError());
 		}
+		// junction annotation of every target slice (src/align.c:688-794: each DP of a spliced mm_align1 gets that of its own
+		// target window), at the slice's offset in a pool parallel to d_pool
+		uint8_t *d_junc = 0;
+		if (P.splice && g.jx.n_seq > 0) {
+			std::vector<wm_junc_win> jw(m);
+			for (int i = 0; i < m; ++i) {
+				const SeqRef &t = jobs[done + perm[i]].t;
+				jw[i].dst_off = dj[i].t_off, jw[i].rid = t.kind == SEQ_REF ? t.rid : -1, jw[i].off = (int32_t)t.off, jw[i].len = t.len, jw[i].reversed = t.reversed;
+			}
+			d_junc = (uint8_t*)g.junc_pool.need(pool_off + 16);
+			wm_junc_win *d_jw = (wm_junc_win*)g.junc_wins.need(sizeof(wm_junc_win) * m);
+			WM_CUDA_CHECK(wm_memcpy_async(d_jw, jw.data(), sizeof(wm_junc_win) * m, cudaMemcpyHostToDevice, st));
+			wm_bed_junc_run(g.jx, d_jw, m, d_junc, st);
+		}
 		int32_t *d_zd = (int32_t*)g.zd.need(sizeof(int32_t) * 5 * (size_t)m);
 		wm_zd_params zp; memset(&zp, 0, sizeof(zp));
 		zp.q = sc.q, zp.e = sc.e; memcpy(zp.mat, sc.mat, 25);
@@ -587,7 +607,7 @@ void GpuBackend::run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin
 			d_coop = (int32_t*)g.coop_ids.need(sizeof(int32_t) * coop.size());
 			WM_CUDA_CHECK(wm_memcpy_async(d_coop, coop.data(), sizeof(int32_t) * coop.size(), cudaMemcpyHostToDevice, st));
 		}
-		wm_extd2_launch(&g.dpws, d_dj, m, plan, d_pool, d_bt, d_ez, d_cig, P, st, &zp, d_zd, d_coop, (int)coop.size(), 0, d_scr);
+		wm_extd2_launch(&g.dpws, d_dj, m, plan, d_pool, d_bt, d_ez, d_cig, P, st, &zp, d_zd, d_coop, (int)coop.size(), d_junc, d_scr);
 		// CIGAR lengths -> offsets -> compacted CIGARs, all behind the traceback on the stream: the host then only copies
 		int32_t *d_nc = (int32_t*)g.nc_buf.need(sizeof(int32_t) * (m + 1));
 		int64_t *d_ooff = (int64_t*)g.cig_off.need(sizeof(int64_t) * (m + 2));
@@ -754,7 +774,19 @@ void gpu_backend_bind(Backend *lane_, const Backend *src_)
 {
 	GpuBackendImpl &g = static_cast<GpuBackend*>(lane_)->g;
 	const GpuBackendImpl &s = static_cast<const GpuBackend*>(src_)->g;
-	g.ix = s.own_ix, g.bf = s.own_bf, g.hidx = s.own_hidx;
+	g.ix = s.own_ix, g.bf = s.own_bf, g.hidx = s.own_hidx, g.jx = s.own_jx;
+}
+
+// Replace the junction intervals of the index `be_` was created with by those of hidx (none when it has no interval with a
+// strand).  Lanes bound to that index see them from their next gpu_backend_bind; no batch may be in flight.
+void gpu_backend_set_junc(Backend *be_, const wm_host_idx *hidx)
+{
+	GpuBackendImpl &g = static_cast<GpuBackend*>(be_)->g;
+	WM_CUDA_CHECK(cudaSetDevice(g.device));
+	WM_CUDA_CHECK(cudaDeviceSynchronize());
+	wm_junc_free(&g.own_jx);
+	g.own_jx = wm_junc_upload(*hidx);
+	g.jx = g.own_jx;
 }
 
 // A second orchestration lane on the same device: shares the resident index, owns its stream and workspaces.
@@ -767,6 +799,7 @@ Backend *gpu_backend_clone(Backend *base_, int n_lanes)
 	g.device = base->g.device; g.hidx = base->g.hidx; g.n_bases = 0;
 	g.ix = base->g.ix; g.bf = base->g.bf;
 	g.own_ix = base->g.own_ix, g.own_bf = base->g.own_bf, g.own_hidx = base->g.own_hidx;
+	g.jx = base->g.jx, g.own_jx = base->g.own_jx;
 	g.st = wm_stream_create_high_priority(); // the DP fill kernels go to a lowest-priority side stream (wm_extd2_launch)
 	g.bt_budget = base->g.bt_budget / (size_t)(n_lanes > 0 ? n_lanes : 1);
 	return be;

@@ -13,6 +13,8 @@ Backend *gpu_backend_create_dev(const wm_host_idx *hidx, uint64_t *d_keys, int64
 void gpu_backend_index_arrays(Backend *be, const uint64_t **d_keys, const uint64_t **d_poff, const uint64_t **d_pos);
 // map with the index another backend was created with (a part of the same multi-part index); streams and workspaces stay
 void gpu_backend_bind(Backend *lane, const Backend *src);
+// the junction intervals of hidx (read_bed_junc / set_junc) on the device, for the index `be` was created with
+void gpu_backend_set_junc(Backend *be, const wm_host_idx *hidx);
 void gpu_backend_destroy(Backend *be);
 }
 

@@ -169,6 +169,8 @@ bool SeqReader::open(const char *fn)
 	return p->fp != 0;
 }
 
+bool SeqReader::next_line(std::string &s) { return p->getline_(s, false); }
+
 // one record with kseq semantics (src/kseq.h): name up to the first white space, rest of the header line is the
 // comment; sequence lines are concatenated; '+' starts the quality of a FASTQ record
 bool SeqReader::next(wm_read &r)

@@ -19,11 +19,17 @@ public:
 	SeqReader(); ~SeqReader();
 	bool open(const char *fn);
 	bool next(wm_read &r);
+	bool next_line(std::string &s); // one line without its \n (and a \r before it, as kseq's KS_SEP_LINE); false at the end
 private:
 	struct Impl; Impl *p;
 };
 
 int read_kmer_list(const char *fn, int k, std::vector<uint64_t> &canon_kmers);
+// mm_idx_bed_read(mi, fn, 1) (src/index.c:690-778): the junction intervals of a BED file (plain or gzip, "-" for stdin) for
+// the sequences of mi, replacing any it had; 0, or -1 when the file cannot be opened (mi is then left as it was)
+int read_bed_junc(wm_host_idx *mi, const char *fn);
+// the same from the reference's mm_idx_t::I (one record per sequence of mi, each sorted by st)
+void set_junc(wm_host_idx *mi, const wm_idx_intv_t *I);
 
 // PAF line of one hit / of an unmapped read (mm_write_paf3, src/format.c:308-334)
 void write_paf(std::string &s, const wm_host_idx *mi, const wm_read *t, const wm_reg1_t *r, int64_t opt_flag, int rep_len);

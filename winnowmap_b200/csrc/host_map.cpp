@@ -162,8 +162,9 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 		fprintf(stderr, "[ERROR] winnowmap-b200: sr/heap-sort modes are outside the accelerated path\n");
 		exit(1);
 	}
-	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR) && mi->junc) { // mm_idx_bed_junc (src/index.c:780) is not built
-		fprintf(stderr, "[ERROR] winnowmap-b200: spliced base-level alignment with junction annotation (--junc-bed) is not supported\n");
+	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR) && mi->junc && !mi->has_junc()) { // WM_IDX_JUNC, but the intervals never came
+		fprintf(stderr, "[ERROR] winnowmap-b200: spliced base-level alignment with junction annotation (--junc-bed) is not supported on an index "
+		        "uploaded with WM_IDX_JUNC until its intervals are set (wm_idx_set_junc or wm_idx_bed_read)\n");
 		exit(1);
 	}
 	// options the reference honours on this path that are not implemented here are refused, not silently ignored

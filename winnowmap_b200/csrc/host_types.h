@@ -61,7 +61,11 @@ typedef wm128_t wm_pair_t; // mm128_t
 struct wm_host_idx {
 	int k, w;
 	int flag = 0;            // mm_idx_t::flag: WM_I_HPC when the index holds homopolymer-compressed minimizers
-	bool junc = false;       // the uploaded index carried junction intervals, which spliced alignment does not read (map_batch refuses)
+	bool junc = false;       // uploaded with WM_IDX_JUNC: the caller's index has junction intervals (map_batch refuses spliced alignment until they are set)
+	// junction intervals (mm_idx_t::I after mm_idx_bed_read, src/index.c:769-778): those of sequence rid at
+	// junc_iv[junc_off[rid] .. junc_off[rid + 1]), sorted by st; junc_off is empty until a BED was read or intervals were set
+	std::vector<wm_idx_intv1_t> junc_iv; std::vector<int64_t> junc_off;
+	bool has_junc() const { return !junc_off.empty(); }
 	std::vector<std::string> name;
 	std::vector<uint32_t> len;
 	std::vector<uint64_t> offset;

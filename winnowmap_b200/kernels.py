@@ -166,6 +166,47 @@ def sdust_batch(seqs, T, W=64):
     return [se[o[i]: o[i + 1]].copy() for i in range(n)]
 
 
+class Intv1(C.Structure):
+    """mm_idx_intv1_t (reference src/index.c): st, en, max, then score:30 and strand:2 in one int32."""
+    _fields_ = [("st", C.c_int32), ("en", C.c_int32), ("max", C.c_int32), ("score", C.c_int32, 30), ("strand", C.c_int32, 2)]
+
+
+class Intv(C.Structure):
+    _fields_ = [("n", C.c_int32), ("m", C.c_int32), ("a", C.POINTER(Intv1))]
+
+
+def intv_records(per_seq):
+    """(array of Intv, keep-alive) from per-sequence lists of (st, en, strand[, score]) tuples, each sorted by st here."""
+    keep, I = [], (Intv * max(1, len(per_seq)))()
+    for r, ivs in enumerate(per_seq):
+        ivs = sorted(ivs, key=lambda x: x[0])
+        a = (Intv1 * max(1, len(ivs)))()
+        for j, v in enumerate(ivs):
+            a[j].st, a[j].en, a[j].max, a[j].strand = int(v[0]), int(v[1]), -1, int(v[2])
+            a[j].score = int(v[3]) if len(v) > 3 else 0
+        keep.append(a)
+        I[r].n, I[r].m, I[r].a = len(ivs), len(ivs), C.cast(a, C.POINTER(Intv1))
+    return I, keep
+
+
+def bed_junc_batch(per_seq, windows):
+    """Batched mm_idx_bed_junc (reference src/index.c:780) on the device.  per_seq: for each sequence, a list of (st, en,
+    strand) intervals (strand 1, -1 or 0); windows: (rid, off, len, reversed) tuples.  Returns one uint8 array per window."""
+    I, keep = intv_records(per_seq)
+    n = len(windows)
+    win = np.array(windows, dtype=np.int32).reshape(n, 4) if n else np.zeros((0, 4), np.int32)
+    out_off = np.zeros(n + 1, dtype=np.int64)
+    if n:
+        out_off[1:] = np.cumsum(win[:, 2])
+    out = np.zeros(int(out_off[-1]) + 1, dtype=np.uint8)
+    L = lib()
+    L.wm_bed_junc_batch.argtypes = [C.POINTER(Intv), C.c_int, C.c_int, i32p, u8p, i64p]
+    if L.wm_bed_junc_batch(I, len(per_seq), n, _p(np.ascontiguousarray(win), i32p), _p(out, u8p), _p(out_off, i64p)) != 0:
+        raise ValueError("wm_bed_junc_batch failed")
+    del keep
+    return [out[out_off[i]: out_off[i + 1]].copy() for i in range(n)]
+
+
 def radix_sort_128x_batch(arrays):
     """radix_sort_128x (reference src/misc.c:156) on each (n,2) uint64 array, tie order included."""
     n = len(arrays)

@@ -42,6 +42,10 @@ def _setup(L):
     if getattr(L, "_wm_mapper_ready", False):
         return L
     L.wm_set_opt.argtypes = [C.c_char_p, C.POINTER(IdxOpt), C.POINTER(MapOpt)]
+    L.wm_idx_bed_read.argtypes = [C.c_void_p, C.c_char_p]
+    L.wm_idx_set_junc.argtypes = [C.c_void_p, C.c_void_p]
+    L.wm_junc_stats.restype = None
+    L.wm_junc_stats.argtypes = [C.POINTER(C.c_double), C.c_int]
     L.wm_check_opt.argtypes = [C.POINTER(IdxOpt), C.POINTER(MapOpt)]
     L.wm_mapopt_max_intron_len.restype = None
     L.wm_mapopt_max_intron_len.argtypes = [C.POINTER(MapOpt), C.c_int]
@@ -151,11 +155,14 @@ class Mapper:
     with sam=True): ksw_exts2 on the GPU, both transcript strands tried per hit, ts:A, introns as N; the other flags of the
     reference (--eqx, --cs, --MD, -u, --splice-flank, -C, --cap-sw-mem) are the fields of self.mo.
     sdust_thres=T is -T: minimizers that lie mostly in low-complexity regions (SDUST with threshold T, window 64) are dropped
-    before seeding, in every stage; 0 (the default) is off.  The command line still refuses -T; the library applies it."""
+    before seeding, in every stage; 0 (the default) is off.  The command line still refuses -T; the library applies it.
+    junc_bed is --junc-bed: a BED file (plain or gzip) of known introns (BED12 blocks, or one interval per line), read into every
+    index part after the index is built.  With spliced_alignment=True every splice DP then adds junc_bonus (self.mo.junc_bonus;
+    9 under splice / cdna, 5 under splice:hq) at annotated donors and acceptors; other mapping is unchanged, as in the reference."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
                  no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None,
-                 splice=False, max_intron_len=None, spliced_alignment=False, sdust_thres=0):
+                 splice=False, max_intron_len=None, spliced_alignment=False, sdust_thres=0, junc_bed=None):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
@@ -191,6 +198,9 @@ class Mapper:
             self.ctx = self.L.wm_index_build_opt(ref.encode(), kmer_freq.encode() if kmer_freq else None, C.byref(self.io), device)
         if not self.ctx:
             raise RuntimeError("index construction failed")
+        if junc_bed is not None and self.L.wm_idx_bed_read(self.ctx, os.fsencode(junc_bed)) != 0:
+            self.close()
+            raise RuntimeError(f"cannot read the BED file {junc_bed!r}")
 
     @property
     def hpc(self):
