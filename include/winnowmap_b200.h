@@ -113,6 +113,23 @@ int wm_sketch_batch_hpc(const wm_bloom_t *bloom, int n, const char *seq, const i
  * and disjoint, at reg[reg_off[i] .. reg_off[i+1]); *reg / *reg_off are malloc()ed by the callee and owned by the caller. */
 int wm_sdust_batch(int n, const char *seq, const int64_t *off, int T, int W, uint64_t **reg, int64_t **reg_off);
 
+/* The seed stage alone (mm_idx_get, collect_matches, skip_seed, then radix_sort_128x or, with heap != 0, the merge of
+ * collect_seed_hits_heap, src/map.c:97-254) on an index given as arrays: keys sorted and unique (minimizer hash, x >> 8),
+ * pos_off the CSR offsets of their occurrence lists in pos (each ascending), seq_len / name_rank per sequence (name_rank: how
+ * many names sort strictly below under strcmp).  Task t's minimizers are mz_xy[mz_off[t] .. mz_off[t+1]) (x, y pairs), its
+ * query length qlen[t]; skip (null: no filter) holds two words per task, the WM seed-filter bits (1 -D, 2 --dual=no,
+ * 4 --for-only, 8 --rev-only, 16 the read's name is an index name) and the number of index names below the read's name.
+ * Output: task t's anchors at (*a_xy)[2 a_off[t] .. 2 a_off[t+1]) (malloc()ed, owned by the caller), rep_len[t],
+ * n_mini_pos[t] and per minimizer mini_pos[m] = position | (kept << 31). */
+int wm_seed_batch(int64_t n_keys, const uint64_t *keys, const uint64_t *pos_off, const uint64_t *pos, int n_seq,
+                  const uint32_t *seq_len, const uint32_t *name_rank, int n_tasks, const uint64_t *mz_xy, const int64_t *mz_off,
+                  const int32_t *qlen, const uint32_t *skip, int max_occ, int heap, uint64_t **a_xy, int64_t **a_off,
+                  int32_t *rep_len, int32_t *n_mini_pos, uint32_t *mini_pos);
+/* Counters of the heap merge on the current device since the last reset: o[0] tasks replayed (those whose sorted anchors
+ * tie), o[1] anchors replayed, o[2] clocks of the merging lanes, o[3] tasks whose heap lay in global memory, o[4] replays that
+ * disagreed with their sorted anchors (always 0).  reset != 0 zeroes them. */
+void wm_seed_heap_stats(double *o, int reset);
+
 /* Batched mm_idx_bed_junc (src/index.c:780-803): the junction annotation of n_win target windows, on the device.  I: n_seq
  * records as wm_idx_bed_read / mm_idx_bed_read leave them (each sorted by st).  Window i is bases [off, off + len) of sequence
  * rid, win[4 i .. 4 i + 3] = (rid, off, len, reversed); reversed gives the bytes in reverse order (mm_seq_rev: the bits are
@@ -362,7 +379,9 @@ wm_gpu_ctx *wm_idx_blob_load(const uint8_t *buf, int64_t size, int device);
  * without a name (qname == 0: only the strand tests apply).  MM_F_SPLICE maps with the cDNA chaining of the reference;
  * with MM_F_CIGAR it also aligns as mm_align_skeleton does for splice (ksw_exts2 on the device, both transcript strands per hit
  * under MM_F_SPLICE_FOR | MM_F_SPLICE_REV, ts:A), with the junction annotation of wm_idx_bed_read / wm_idx_set_junc when the
- * context has intervals.  MM_F_SR and MM_F_HEAP_SORT are refused. */
+ * context has intervals.  MM_F_HEAP_SORT (--heap-sort=yes) collects every stage's anchors in the order of
+ * collect_seed_hits_heap (src/map.c:156-220): the tasks whose sorted anchors tie are replayed through the heap on the device.
+ * MM_F_SR is refused. */
 int wm_gpu_map_batch(wm_gpu_ctx *ctx, const wm_mapopt_t *opt, int n_seq, const char *const *names, const char *const *seqs,
                      const int32_t *lens, int32_t *n_reg, wm_reg1_t **reg, int32_t *rep_len, int32_t *frag_gap, int n_threads);
 

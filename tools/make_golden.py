@@ -898,6 +898,103 @@ def main_sdust():
     json.dump(manifest, open(os.path.join(gdir, "sdust_manifest.json"), "w"), indent=1, sort_keys=True)
 
 
+# ---- heap sort (--heap-sort=yes): tests/golden/heap_manifest.json and heap_*; the other manifests are not touched ----
+# Short-unit tandem data: a random reference with 40 tandem arrays of 5-40 copies of 15-120 bp units at 2 % divergence, and 300
+# reads of 2-20 kb at 5 % error from it, half reverse-complemented ("tandem"; "tandem_ava": the first 60 reads against themselves).
+# Copies of one query hash share an occurrence list, so their anchors tie in x and the heap's order differs from the sort's.
+HEAP_CASES = {
+    # name: (inputs, reference options, library options of Mapper)
+    "heap_tandem_c": ("tandem", ["-x", "map-ont", "-c"], dict(preset="map-ont")),
+    "heap_tandem_pb": ("tandem", ["-x", "map-pb", "-c"], dict(preset="map-pb")),
+    "heap_tandem_a": ("tandem", ["-x", "map-ont", "-a"], dict(preset="map-ont", sam=True)),
+    "heap_tandem_H": ("tandem", ["-x", "map-ont", "-H", "-c"], dict(preset="map-ont", hpc=True)),
+    "heap_tandem_I_split": ("tandem", ["-x", "map-ont", "-c", "-I", "150000", "--split-prefix", "SPLIT"],
+                            dict(preset="map-ont", part_bases=150000, split=True)),
+    "heap_tandem_X": ("tandem_ava", ["-x", "map-ont", "-X", "-c"], dict(preset="map-ont", all_vs_all=True)),
+    "heap_splice": ("tx", ["-x", "splice"], dict(preset="splice", cigar=False)),
+}
+
+
+def make_heap_inputs(inputs, outdir):
+    """(index FASTA, reads FASTA) of one heap-sort input set."""
+    if inputs == "tx":
+        ref, reads, _ = make_splice_inputs("tx", outdir)
+        return ref, reads
+    os.makedirs(outdir, exist_ok=True)
+    ref, reads = os.path.join(outdir, "heap_tandem.ref.fa"), os.path.join(outdir, "heap_tandem.reads.fa")
+    rng = np.random.default_rng(11)
+    A = np.frombuffer(b"ACGT", dtype=np.uint8)
+
+    def rs(n):
+        return A[rng.integers(0, 4, n)]
+
+    def mutate(s, e):
+        r = rng.random(len(s))
+        sub = A[rng.integers(0, 4, len(s))]
+        ins = A[rng.integers(0, 4, len(s))]
+        out = []
+        for c, x, b1, b2 in zip(s.tolist(), r.tolist(), sub.tolist(), ins.tolist()):
+            if x < e * 0.6:
+                out.append(b1)
+            elif x < e * 0.8:
+                continue
+            elif x < e:
+                out += (c, b2)
+            else:
+                out.append(c)
+        return np.array(out, dtype=np.uint8)
+
+    parts = [rs(50000)]
+    for _ in range(40):
+        u = rs(int(rng.integers(15, 120)))
+        parts += [mutate(u, 0.02) for _ in range(int(rng.integers(5, 40)))] + [rs(int(rng.integers(2000, 8000)))]
+    g = np.concatenate(parts)
+    with open(ref, "w") as f:
+        f.write(">c1\n" + g.tobytes().decode() + "\n")
+    comp = bytes.maketrans(b"ACGT", b"TGCA")
+    ava = os.path.join(outdir, "heap_tandem_ava.reads.fa")
+    with open(reads, "w") as f, open(ava, "w") as fa:
+        for i in range(300):
+            L = int(rng.integers(2000, 20000))
+            p = int(rng.integers(0, len(g) - L))
+            r = mutate(g[p:p + L], 0.05).tobytes()
+            if rng.random() < 0.5:
+                r = r.translate(comp)[::-1]
+            f.write(f">r{i}\n{r.decode()}\n")
+            if i < 60:
+                fa.write(f">r{i}\n{r.decode()}\n")
+    return (ava, ava) if inputs == "tandem_ava" else (ref, reads)
+
+
+def main_heap():
+    refbin = os.path.join(ROOT, "oracle", "_ref", "winnowmap")
+    if not os.path.exists(refbin):
+        subprocess.check_call([os.path.join(ROOT, "oracle", "build_ref.sh")])
+    gdir = os.path.join(ROOT, "tests", "golden")
+    tmp = "/tmp/wm_golden_heap"
+    manifest = {}
+    for name, (inputs, args, lib_opts) in HEAP_CASES.items():
+        ref, reads = make_heap_inputs(inputs, tmp)
+        outs = []
+        for hs in ("yes", "no"):
+            a = [x if x != "SPLIT" else os.path.join(tmp, name + ".split") for x in args]
+            cmd = [refbin, "-t", "8"] + a + ["--heap-sort=" + hs, ref, reads]
+            outs.append(subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, check=True).stdout)
+        sam = "-a" in args
+        out, out0 = (sam_without_pg(o) if sam else o for o in outs)
+        with gzip.GzipFile(os.path.join(gdir, name + (".sam.stripped.gz" if sam else ".paf.gz")), "wb", mtime=0) as f:
+            f.write(sam_strip_seq(out) if sam else out)
+        manifest[name] = dict(inputs=inputs, lib=lib_opts, sam=sam, ref_md5=md5(ref), reads_md5=md5(reads),
+                              # not "cmd": the command-line parse check replays every "cmd" of the manifests, and the command line
+                              # refuses --heap-sort=yes
+                              ref_cmd=" ".join(["winnowmap"] + [x if x != "SPLIT" else "<prefix>" for x in args] +
+                                               ["--heap-sort=yes", "ref.fa", "reads.fa"]),
+                              out_md5=hashlib.md5(out).hexdigest(), n_lines=out.count(b"\n"),
+                              n_lines_differing=len(set(out.split(b"\n")) ^ set(out0.split(b"\n"))))
+        print(name, manifest[name]["n_lines"], "lines,", manifest[name]["n_lines_differing"], "differ from --heap-sort=no", flush=True)
+    json.dump(manifest, open(os.path.join(gdir, "heap_manifest.json"), "w"), indent=1, sort_keys=True)
+
+
 # ---- junction annotation (--junc-bed with spliced base-level alignment): tests/golden/splice_junc_manifest.json and splice_junc_*;
 # the other manifests are not touched.  The inputs are those of the splice_aln_* cases plus a BED of the transcriptome: "full" lists
 # every transcript (isoforms and paralogs included) as BED12 with the gene's strand, "mixed" (gzipped) half of them as BED12 and
@@ -1037,7 +1134,9 @@ def record_junc_intervals(tmp, gdir):
 
 
 if __name__ == "__main__":
-    if "--junc" in sys.argv:
+    if "--heap" in sys.argv:
+        main_heap()
+    elif "--junc" in sys.argv:
         main_junc()
     elif "--sdust" in sys.argv:
         main_sdust()

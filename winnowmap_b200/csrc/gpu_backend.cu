@@ -100,6 +100,7 @@ struct GpuBackendImpl {
 	// workspaces
 	wm_sketch_ws sk; wm_seed_ws sd, sd2; wm_chain_ws ch; wm_extd2_ws dpws;
 	int sdust_T = 0; wm_sdust_ws sdw; // -T (0: off; sdw is then never touched)
+	bool heap_sort = false;            // --heap-sort=yes
 	wm_dbuf masked_pk, masked_nm, mask_tasks, mask_toff, mask_pool, qlen_buf, skip_buf, pre_buf, cat_tasks, cat_toff, cat_a, set_id, off_buf, nb_off, nu_off, b_out, u_out;
 	wm_dbuf nc_buf, scan_tmp, coop_ids, g_jobs, g_joff, seq_pool, dp_jobs, bt, ez, cig, cig_off, cig_out, ll_jobs, ll_scr, ll_out, mat;
 	// host result pools
@@ -142,6 +143,7 @@ public:
 	void begin_batch(const std::vector<const wm_read*> &reads) override;
 	void set_resident_pool(const char *device_ascii) override { g.resident_pool = device_ascii; }
 	bool set_sdust(int T) override { g.sdust_T = T > 0 ? T : 0; return true; }
+	bool set_heap_sort(bool on) override { g.heap_sort = on; return true; }
 	void seed_chain(const std::vector<SeedTask> &tasks, const int32_t *mask_pool, const wm_pair_t *pre_pool, const ChainParams cp[2], int max_occ, std::vector<SeedOut> &out) override;
 	void run_dp(const std::vector<DpJob> &jobs, const std::vector<MapWin> &wins, const DpScoring &sc, std::vector<DpRes> &res) override;
 	void run_ll(const std::vector<LlJob> &jobs, const std::vector<MapWin> &wins, const DpScoring &sc, std::vector<LlRes> &res) override;
@@ -286,7 +288,7 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 			WM_CUDA_CHECK(wm_memcpy_async(d_skip, skip.data(), sizeof(uint2) * ns, cudaMemcpyHostToDevice, st));
 		}
 		std::vector<int64_t> a_off(ns + 1);
-		wm_seed_run(sdp[pass], g.ix, (const wm128_dev*)g.sk.mz.p, (const int64_t*)g.sk.mz_off.p, n_mz, ns, d_qlen, max_occ, a_off.data(), st, d_skip);
+		wm_seed_run(sdp[pass], g.ix, (const wm128_dev*)g.sk.mz.p, (const int64_t*)g.sk.mz_off.p, n_mz, ns, d_qlen, max_occ, a_off.data(), st, d_skip, g.heap_sort);
 		d_seed_a[pass] = (wm128_dev*)sdp[pass]->a.p;
 		// small per-task results
 		std::vector<int32_t> rep(ns);
@@ -302,6 +304,7 @@ void GpuBackend::seed_chain(const std::vector<SeedTask> &tasks, const int32_t *m
 		}
 		wm_stream_sync(st);
 		if (g.sdust_T > 0) wm_sdust_check(&g.sdw);
+		if (g.heap_sort) wm_seed_heap_check();
 		for (int i = 0; i < ns; ++i) {
 			const int t = ids[i];
 			g.h_rep[t] = rep[i];

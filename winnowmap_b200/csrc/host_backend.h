@@ -67,6 +67,9 @@ public:
 	// -T: the SDUST threshold of the next seed_chain calls (0: off).  Returns whether the backend applies it; one that cannot
 	// keeps the default, and map_batch refuses T > 0 on it instead of mapping as if T were 0.
 	virtual bool set_sdust(int T) { (void)T; return false; }
+	// --heap-sort: whether the next seed_chain calls collect anchors in the order of collect_seed_hits_heap (src/map.c:156-220)
+	// instead of collect_seed_hits.  Returns whether the backend applies it; map_batch refuses heap sort on one that cannot.
+	virtual bool set_heap_sort(bool on) { (void)on; return false; }
 	virtual void seed_chain(const std::vector<SeedTask> &tasks, const int32_t *mask_pool, const wm_pair_t *pre_pool,
 	                        const ChainParams cp[2], int max_occ, std::vector<SeedOut> &out) = 0;
 	// `wins[job.task]` locates the query window of each job

@@ -158,8 +158,13 @@ void map_batch(Backend *be, const wm_host_idx *mi, const wm_mapopt_t *opt, const
 	frag_gap_out.assign(n_reads, 0);
 	if (n_reads == 0) return;
 	if (n_threads < 1) n_threads = 1;
-	if (opt->flag & (WM_F_SR | WM_F_HEAP_SORT)) {
-		fprintf(stderr, "[ERROR] winnowmap-b200: sr/heap-sort modes are outside the accelerated path\n");
+	if (opt->flag & WM_F_SR) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: sr mode is outside the accelerated path\n");
+		exit(1);
+	}
+	// --heap-sort=yes: every seed collection of the three stages (src/map.c:363, :535, :810, :860) merges the occurrence lists
+	if (!be->set_heap_sort((opt->flag & WM_F_HEAP_SORT) != 0) && (opt->flag & WM_F_HEAP_SORT)) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: this backend does not apply heap sort (--heap-sort=yes)\n");
 		exit(1);
 	}
 	if ((opt->flag & WM_F_SPLICE) && (opt->flag & WM_F_CIGAR) && mi->junc && !mi->has_junc()) { // WM_IDX_JUNC, but the intervals never came

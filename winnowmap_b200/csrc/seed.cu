@@ -6,6 +6,7 @@
 // `pos_off` into the occurrence array `pos` (each list ascending, as src/index.c:239 leaves it) and an
 // open-addressing hash table key -> key index for O(1) probes.  The bucket/khash structure of the
 // reference is an implementation detail; the contract "hash -> (sorted list, n)" is what is kept.
+#include <string.h>
 #include <vector>
 #include <algorithm>
 #include "wm_common.cuh"
@@ -13,6 +14,7 @@
 #include "sketch.cuh"
 #include "rsort.cuh"
 #include "seed.cuh"
+#include "seed_heap.cuh"
 
 #define WM_HT_EMPTY 0xffffffffffffffffULL
 
@@ -89,36 +91,10 @@ __global__ void wm_seed_expand_kernel(wm_idx_dev ix, const wm128_dev *__restrict
 	while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (a_off[mid] <= j) lo = mid; else hi = mid; }
 	const wm128_dev p = mz[lo];
 	const uint64_t r = ix.pos[list_off[lo] + (uint64_t)(j - a_off[lo])];
-	const uint32_t q_pos = (uint32_t)p.y, q_span = (uint32_t)(p.x & 0xff);
-	const int32_t rpos = (uint32_t)r >> 1;
 	wm128_dev o;
-	if ((r & 1) == (q_pos & 1)) { // forward strand
-		o.x = (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
-		o.y = (uint64_t)q_span << 32 | q_pos >> 1;
-	} else { // reverse strand
-		o.x = 1ULL << 63 | (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
-		o.y = (uint64_t)q_span << 32 | (uint32_t)(qlen[mz_task[lo]] - ((q_pos >> 1) + 1 - q_span) - 1);
-	}
-	o.y |= (uint64_t)(p.y >> 32) << 48; // MM_SEED_SEG_SHIFT
-	if (tandem[lo]) o.y |= 1ULL << 42;   // MM_SEED_TANDEM
-	if (FILTER) {
-		const int t = mz_task[lo];
-		const uint2 sk = skip[t];
-		const bool fwd = (r & 1) == (q_pos & 1);
-		bool drop = false;
-		if (sk.x & (WM_SKIP_NO_DIAG | WM_SKIP_NO_DUAL)) {
-			const uint32_t rid = (uint32_t)(r >> 32), rank = ix.name_rank[rid];
-			// strcmp(qname, name) == 0 and the sequence is as long as the window (not the read: src/map.c:364, :813)
-			if ((sk.x & WM_SKIP_NO_DIAG) && (sk.x & WM_SKIP_NAME_EQ) && rank == sk.y && (int)ix.seq_len[rid] == qlen[t]) {
-				if ((uint32_t)rpos == q_pos >> 1) drop = true; // the diagonal
-				else if (fwd) o.y |= 1ULL << 43;              // MM_SEED_SELF
-			}
-			if ((sk.x & WM_SKIP_NO_DUAL) && rank < sk.y) drop = true; // strcmp(qname, name) > 0
-		}
-		if ((sk.x & WM_SKIP_FOR_ONLY) && !fwd) drop = true;
-		if ((sk.x & WM_SKIP_REV_ONLY) && fwd) drop = true;
-		keep[j] = drop ? 0 : 1;
-	}
+	bool drop = false;
+	WM_SEED_ANCHOR(FILTER, ix, p, r, qlen, skip, mz_task[lo], tandem[lo], o, drop);
+	if (FILTER) keep[j] = drop ? 0 : 1;
 	a[j] = o;
 }
 
@@ -740,12 +716,133 @@ void wm_anchor_sort_run(wm_seed_ws *ws, wm128_dev *d_a, const int64_t *d_off, co
 	}
 }
 
+// ---- --heap-sort=yes: collect_seed_hits_heap for the tasks whose sorted anchors tie (seed_heap.cuh) ----
+// tie scan: one thread per sorted anchor; the first thread to see a[j].x == a[j - 1].x inside task t lists t
+__global__ void wm_seed_tie_scan_kernel(const wm128_dev *__restrict__ a, const int64_t *__restrict__ task_a_off, int n_tasks, int64_t n_a,
+                                        int32_t *__restrict__ flag, int32_t *__restrict__ ids, int32_t *__restrict__ n_ids)
+{
+	const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= n_a || j == 0) return;
+	if (a[j].x != a[j - 1].x) return;
+	int lo = 0, hi = n_tasks; // the task holding j: last t with task_a_off[t] <= j
+	while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (task_a_off[mid] <= j) lo = mid; else hi = mid; }
+	if (j == task_a_off[lo]) return; // the previous anchor belongs to another task
+	if (atomicCAS(&flag[lo], 0, 1) == 0) ids[atomicAdd(n_ids, 1)] = lo;
+}
+
+// counters of the replay, summed over all launches on a device (wm_seed_heap_stats): tasks, anchors, clocks of the merging
+// lane, tasks whose heap lay in global memory, tasks whose replay disagreed with their sorted slice
+__device__ unsigned long long g_wm_heap_stat[5];
+
+// heap replay: one warp per listed task.  A task takes this launch when its heap, lists and staged occurrences need at most
+// smem_bytes (small launch: min_bytes 0) or more than min_bytes (large launch: heap and lists in shared memory when they fit,
+// the occurrences too when those fit as well; else both in global memory, heap_g / list_g at the task's minimizer offsets).
+template <bool FILTER>
+__global__ void __launch_bounds__(32)
+wm_seed_heap_kernel(wm_idx_dev ix, const wm128_dev *__restrict__ mz, const int64_t *__restrict__ mz_off, const int32_t *__restrict__ cnt,
+                    const uint64_t *__restrict__ list_off, const uint8_t *__restrict__ tandem, const int64_t *__restrict__ raw_off,
+                    const int32_t *__restrict__ qlen, const uint2 *__restrict__ skip, const int32_t *__restrict__ ids, const int32_t *__restrict__ n_ids,
+                    const int64_t *__restrict__ task_a_off, wm128_dev *__restrict__ a, wm128_dev *heap_g, wm_heap_list *list_g,
+                    int64_t smem_bytes, int64_t min_bytes)
+{
+	extern __shared__ __align__(16) unsigned char wm_heap_smem[];
+	const int lane = threadIdx.x, n_t = *n_ids;
+	for (int i = blockIdx.x; i < n_t; i += gridDim.x) {
+		const int t = ids[i];
+		const int64_t m0 = mz_off[t], m1 = mz_off[t + 1], nm = m1 - m0, n_raw = raw_off[m1] - raw_off[m0];
+		const int64_t hl = nm * (int64_t)WM_HEAP_ENTRY_BYTES, need = hl + n_raw * (int64_t)sizeof(uint64_t);
+		if (min_bytes == 0 ? need > smem_bytes : need <= min_bytes) continue; // the other launch's task
+		wm128_dev *H; wm_heap_list *L; uint64_t *stage = 0;
+		const bool in_smem = hl <= smem_bytes;
+		if (in_smem) {
+			H = (wm128_dev*)wm_heap_smem, L = (wm_heap_list*)(H + nm);
+			if (need <= smem_bytes) stage = (uint64_t*)(L + nm);
+		} else H = heap_g + m0, L = list_g + m0;
+		const int64_t base = task_a_off[t], n = task_a_off[t + 1] - base;
+		const long long c0 = clock64();
+		const int64_t w = wm_heap_replay_task<FILTER>(ix, mz, m0, m1, cnt, list_off, tandem, raw_off, qlen[t], FILTER ? skip[t] : make_uint2(0, 0),
+		                                              H, L, stage, a + base, n, lane);
+		if (lane == 0) {
+			atomicAdd(&g_wm_heap_stat[0], 1ULL); atomicAdd(&g_wm_heap_stat[1], (unsigned long long)n);
+			atomicAdd(&g_wm_heap_stat[2], (unsigned long long)(clock64() - c0));
+			if (!in_smem) atomicAdd(&g_wm_heap_stat[3], 1ULL);
+			if (w != n) atomicAdd(&g_wm_heap_stat[4], 1ULL);
+		}
+		__syncwarp();
+	}
+}
+
+#define WM_HEAP_SMEM_SMALL (24 << 10)  // the small launch: up to nine CTAs per SM
+#define WM_HEAP_SMEM_LARGE (200 << 10) // the large launch: one CTA per SM
+
+// after the seed pass of heap sort: lists the tasks with ties and replays them.  h_mz_off: host copy of mz_off.
+static void wm_seed_heap_run(wm_seed_ws *ws, const wm_idx_dev &ix, const wm128_dev *d_mz, const int64_t *d_mz_off, const int64_t *h_mz_off,
+                             int n_tasks, const int32_t *d_qlen, const uint2 *d_skip, wm128_dev *d_a, const int64_t *d_task_a_off, cudaStream_t st)
+{
+	const int64_t n_a = ws->n_a;
+	if (n_a < 2) return;
+	int32_t *d_flag = (int32_t*)ws->heap_flag.need(sizeof(int32_t) * (n_tasks + 1));
+	int32_t *d_ids = (int32_t*)ws->heap_ids.need(sizeof(int32_t) * (n_tasks + 1));
+	WM_CUDA_CHECK(cudaMemsetAsync(d_flag, 0, sizeof(int32_t) * (n_tasks + 1), st)); // d_flag[n_tasks]: the list's length
+	wm_count_launch(); wm_seed_tie_scan_kernel<<<(unsigned)((n_a + 255) / 256), 256, 0, st>>>(d_a, d_task_a_off, n_tasks, n_a, d_flag, d_ids, d_flag + n_tasks);
+	WM_CUDA_CHECK(cudaGetLastError());
+	int64_t max_nm = 0; // the heap in global memory: only for tasks whose heap and lists outgrow the large launch's shared memory
+	for (int t = 0; t < n_tasks; ++t) max_nm = std::max(max_nm, h_mz_off[t + 1] - h_mz_off[t]);
+	wm128_dev *heap_g = 0; wm_heap_list *list_g = 0;
+	if (max_nm * (int64_t)WM_HEAP_ENTRY_BYTES > WM_HEAP_SMEM_LARGE) {
+		heap_g = (wm128_dev*)ws->heap_g.need(sizeof(wm128_dev) * (h_mz_off[n_tasks] + 1));
+		list_g = (wm_heap_list*)ws->heap_l.need(sizeof(wm_heap_list) * (h_mz_off[n_tasks] + 1));
+	}
+	static bool attr_set = false;
+	if (!attr_set) {
+		WM_CUDA_CHECK(cudaFuncSetAttribute(wm_seed_heap_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WM_HEAP_SMEM_LARGE));
+		WM_CUDA_CHECK(cudaFuncSetAttribute(wm_seed_heap_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WM_HEAP_SMEM_LARGE));
+		attr_set = true;
+	}
+	const int sms = wm_sm_count();
+	const int64_t *d_raw = (const int64_t*)ws->a_off.p;
+	const int32_t *d_cnt = (const int32_t*)ws->cnt.p;
+	const uint64_t *d_loff = (const uint64_t*)ws->list_off.p;
+	const uint8_t *d_td = (const uint8_t*)ws->tandem.p;
+	const unsigned g_s = (unsigned)std::min(n_tasks, 9 * sms), g_l = (unsigned)std::min(n_tasks, sms);
+	for (int cls = 0; cls < 2; ++cls) {
+		const int64_t smem = cls == 0 ? WM_HEAP_SMEM_SMALL : WM_HEAP_SMEM_LARGE, min_b = cls == 0 ? 0 : WM_HEAP_SMEM_SMALL;
+		const unsigned g = cls == 0 ? g_s : g_l;
+		wm_count_launch();
+		if (d_skip) wm_seed_heap_kernel<true><<<g, 32, smem, st>>>(ix, d_mz, d_mz_off, d_cnt, d_loff, d_td, d_raw, d_qlen, d_skip, d_ids, d_flag + n_tasks,
+		                                                           d_task_a_off, d_a, heap_g, list_g, smem, min_b);
+		else wm_seed_heap_kernel<false><<<g, 32, smem, st>>>(ix, d_mz, d_mz_off, d_cnt, d_loff, d_td, d_raw, d_qlen, 0, d_ids, d_flag + n_tasks,
+		                                                     d_task_a_off, d_a, heap_g, list_g, smem, min_b);
+		WM_CUDA_CHECK(cudaGetLastError());
+	}
+}
+
+// stats of the replay on the current device: o[0..4] = g_wm_heap_stat (see above); reset: zero them
+extern "C" void wm_seed_heap_stats(double *o, int reset)
+{
+	unsigned long long h[5];
+	WM_CUDA_CHECK(cudaMemcpyFromSymbol(h, g_wm_heap_stat, sizeof(h)));
+	for (int i = 0; i < 5; ++i) o[i] = (double)h[i];
+	if (reset) { memset(h, 0, sizeof(h)); WM_CUDA_CHECK(cudaMemcpyToSymbol(g_wm_heap_stat, h, sizeof(h))); }
+}
+
+// a replay that disagreed with its task's sorted slice cannot happen; if one did, the anchors are wrong and must not pass
+void wm_seed_heap_check(void)
+{
+	unsigned long long bad = 0;
+	WM_CUDA_CHECK(cudaMemcpyFromSymbol(&bad, g_wm_heap_stat, sizeof(bad), 4 * sizeof(unsigned long long)));
+	if (bad) {
+		fprintf(stderr, "[ERROR] winnowmap-b200: the heap merge of %llu seed task(s) disagreed with their sorted anchors\n", bad);
+		exit(1);
+	}
+}
+
 // Collect sorted anchors for all sketched tasks.  Inputs are the outputs of wm_sketch_run.
 // On return: ws->a (anchors), ws->task_a_off (device, n_tasks+1), ws->rep_len, ws->n_mini_pos, ws->mini_pos;
 // h_task_a_off (host, n_tasks+1) receives the anchor offsets.
 void wm_seed_run(wm_seed_ws *ws, const wm_idx_dev &ix, const wm128_dev *d_mz, const int64_t *d_mz_off, int64_t n_mz, int n_tasks,
-                 const int32_t *d_qlen, int max_occ, int64_t *h_task_a_off, cudaStream_t st, const uint2 *d_skip)
-{ // d_skip: the seed filter's bits per task, or null when no task filters (then no filter kernel runs)
+                 const int32_t *d_qlen, int max_occ, int64_t *h_task_a_off, cudaStream_t st, const uint2 *d_skip, bool heap)
+{ // d_skip: the seed filter's bits per task, or null when no task filters (then no filter kernel runs); heap: --heap-sort=yes
 	for (int i = 0; i <= n_tasks; ++i) h_task_a_off[i] = 0;
 	int64_t *d_task_a_off = (int64_t*)ws->task_a_off.need(sizeof(int64_t) * (n_tasks + 1));
 	int32_t *d_rep = (int32_t*)ws->rep_len.need(sizeof(int32_t) * (n_tasks + 1));
@@ -800,6 +897,12 @@ void wm_seed_run(wm_seed_ws *ws, const wm_idx_dev &ix, const wm128_dev *d_mz, co
 	wm_stream_sync(st);
 	ws->n_a = h_task_a_off[n_tasks];
 	wm_anchor_sort_run(ws, d_a, d_task_a_off, h_task_a_off, n_tasks, st);
+	if (heap) {
+		std::vector<int64_t> h_mz_off(n_tasks + 1);
+		WM_CUDA_CHECK(wm_memcpy_async(h_mz_off.data(), d_mz_off, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyDeviceToHost, st));
+		wm_stream_sync(st);
+		wm_seed_heap_run(ws, ix, d_mz, d_mz_off, h_mz_off.data(), n_tasks, d_qlen, d_skip, d_a, d_task_a_off, st);
+	}
 }
 
 // ---- index upload ----
@@ -837,5 +940,60 @@ extern "C" int wm_radix_sort_128x_batch(int n_arr, wm128_dev *a, const int64_t *
 	WM_CUDA_CHECK(cudaMemcpy(a, d_a, sizeof(wm128_dev) * n, cudaMemcpyDeviceToHost));
 	ws.release();
 	cudaFree(d_a); cudaFree(d_off);
+	return 0;
+}
+
+// ---- C ABI: the seed stage alone (lookup, anchors, seed filter, tie-exact sort and, with heap, the heap merge), on an index given
+// as arrays, for the parity tests ----
+extern "C" int wm_seed_batch(int64_t n_keys, const uint64_t *keys, const uint64_t *pos_off, const uint64_t *pos, int n_seq,
+                             const uint32_t *seq_len, const uint32_t *name_rank, int n_tasks, const uint64_t *mz_xy, const int64_t *mz_off,
+                             const int32_t *qlen, const uint32_t *skip, int max_occ, int heap, uint64_t **a_xy, int64_t **a_off,
+                             int32_t *rep_len, int32_t *n_mini_pos, uint32_t *mini_pos)
+{
+	int ndev = 0;
+	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+		fprintf(stderr, "[ERROR] wm_seed_batch: no CUDA device visible; winnowmap-b200 has no CPU fallback\n");
+		exit(1);
+	}
+	*a_off = (int64_t*)calloc(n_tasks + 1, sizeof(int64_t));
+	*a_xy = (uint64_t*)malloc(16);
+	if (n_tasks <= 0) return 0;
+	const int64_t n_mz = mz_off[n_tasks], n_pos = pos_off[n_keys];
+	wm_idx_dev ix;
+	memset(&ix, 0, sizeof(ix));
+	ix.n_keys = n_keys, ix.n_seq = (uint32_t)n_seq;
+	uint64_t *d_keys = wm_dev_alloc<uint64_t>(n_keys + 1), *d_poff = wm_dev_alloc<uint64_t>(n_keys + 1), *d_pos = wm_dev_alloc<uint64_t>(n_pos + 1);
+	uint32_t *d_len = wm_dev_alloc<uint32_t>(n_seq + 1), *d_rank = wm_dev_alloc<uint32_t>(n_seq + 1);
+	if (n_keys > 0) WM_CUDA_CHECK(cudaMemcpy(d_keys, keys, sizeof(uint64_t) * n_keys, cudaMemcpyHostToDevice));
+	WM_CUDA_CHECK(cudaMemcpy(d_poff, pos_off, sizeof(uint64_t) * (n_keys + 1), cudaMemcpyHostToDevice));
+	if (n_pos > 0) WM_CUDA_CHECK(cudaMemcpy(d_pos, pos, sizeof(uint64_t) * n_pos, cudaMemcpyHostToDevice));
+	if (n_seq > 0) {
+		WM_CUDA_CHECK(cudaMemcpy(d_len, seq_len, sizeof(uint32_t) * n_seq, cudaMemcpyHostToDevice));
+		WM_CUDA_CHECK(cudaMemcpy(d_rank, name_rank, sizeof(uint32_t) * n_seq, cudaMemcpyHostToDevice));
+	}
+	ix.keys = d_keys, ix.pos_off = d_poff, ix.pos = d_pos, ix.seq_len = d_len, ix.name_rank = d_rank;
+	wm_idx_dev_build_ht(&ix, 0);
+	wm128_dev *d_mz = wm_dev_alloc<wm128_dev>(n_mz + 1);
+	int64_t *d_mzoff = wm_dev_alloc<int64_t>(n_tasks + 1);
+	int32_t *d_qlen = wm_dev_alloc<int32_t>(n_tasks);
+	uint2 *d_skip = skip ? wm_dev_alloc<uint2>(n_tasks) : 0;
+	if (n_mz > 0) WM_CUDA_CHECK(cudaMemcpy(d_mz, mz_xy, sizeof(wm128_dev) * n_mz, cudaMemcpyHostToDevice));
+	WM_CUDA_CHECK(cudaMemcpy(d_mzoff, mz_off, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyHostToDevice));
+	WM_CUDA_CHECK(cudaMemcpy(d_qlen, qlen, sizeof(int32_t) * n_tasks, cudaMemcpyHostToDevice));
+	if (skip) WM_CUDA_CHECK(cudaMemcpy(d_skip, skip, sizeof(uint2) * n_tasks, cudaMemcpyHostToDevice));
+	wm_seed_ws ws;
+	wm_seed_run(&ws, ix, d_mz, d_mzoff, n_mz, n_tasks, d_qlen, max_occ, *a_off, 0, d_skip, heap != 0);
+	WM_CUDA_CHECK(cudaDeviceSynchronize());
+	if (heap) wm_seed_heap_check();
+	const int64_t n_a = (*a_off)[n_tasks];
+	free(*a_xy);
+	*a_xy = (uint64_t*)malloc(sizeof(wm128_dev) * (n_a + 1));
+	if (n_a > 0) WM_CUDA_CHECK(cudaMemcpy(*a_xy, ws.a.p, sizeof(wm128_dev) * n_a, cudaMemcpyDeviceToHost));
+	WM_CUDA_CHECK(cudaMemcpy(rep_len, ws.rep_len.p, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost));
+	WM_CUDA_CHECK(cudaMemcpy(n_mini_pos, ws.n_mini_pos.p, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost));
+	if (n_mz > 0) WM_CUDA_CHECK(cudaMemcpy(mini_pos, ws.mini_pos.p, sizeof(uint32_t) * n_mz, cudaMemcpyDeviceToHost));
+	ws.release();
+	cudaFree(d_keys); cudaFree(d_poff); cudaFree(d_pos); cudaFree(d_len); cudaFree(d_rank); cudaFree((void*)ix.ht_key); cudaFree((void*)ix.ht_val);
+	cudaFree(d_mz); cudaFree(d_mzoff); cudaFree(d_qlen); cudaFree(d_skip);
 	return 0;
 }

@@ -166,6 +166,57 @@ def sdust_batch(seqs, T, W=64):
     return [se[o[i]: o[i + 1]].copy() for i in range(n)]
 
 
+def seed_batch(keys, pos_off, pos, tasks, max_occ, heap=False, seq_len=None, name_rank=None, skip=None):
+    """The seed stage alone on the device (wm_seed_batch): mm_idx_get, collect_matches, skip_seed and radix_sort_128x, or with
+    heap=True the order of collect_seed_hits_heap (reference src/map.c:97-254).  The index: keys (sorted unique hashes), pos_off
+    (CSR offsets, len(keys) + 1) and pos (occurrences, each list ascending); seq_len / name_rank per index sequence (for the
+    filter).  tasks: list of (mz_xy (n, 2) uint64, qlen).  skip: None, or per task (WM seed-filter bits, names below the read's).
+    Returns per task (anchors (n, 2) uint64, rep_len, n_mini_pos, mini_pos uint32 per minimizer: position | kept << 31)."""
+    L = lib()
+    L.wm_seed_batch.argtypes = [C.c_int64, u64p, u64p, u64p, C.c_int, u32p, u32p, C.c_int, u64p, i64p, i32p, u32p, C.c_int, C.c_int,
+                                C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), i32p, i32p, u32p]
+    keys = np.ascontiguousarray(keys, dtype=np.uint64)
+    pos_off = np.ascontiguousarray(pos_off, dtype=np.uint64)
+    pos = np.ascontiguousarray(pos, dtype=np.uint64)
+    if len(pos) == 0:
+        pos = np.zeros(1, np.uint64)
+    n_seq = 0 if seq_len is None else len(seq_len)
+    seq_len = np.ascontiguousarray(seq_len if seq_len is not None else [0], dtype=np.uint32)
+    name_rank = np.ascontiguousarray(name_rank if name_rank is not None else [0], dtype=np.uint32)
+    n = len(tasks)
+    mz_off = np.zeros(n + 1, dtype=np.int64)
+    mz_off[1:] = np.cumsum([len(t[0]) for t in tasks])
+    mz = np.ascontiguousarray(np.concatenate([np.asarray(t[0], dtype=np.uint64).reshape(-1, 2) for t in tasks] + [np.zeros((1, 2), np.uint64)]))
+    qlen = np.ascontiguousarray([t[1] for t in tasks] + [0], dtype=np.int32)
+    sk = None if skip is None else np.ascontiguousarray(np.asarray(skip, dtype=np.uint32).reshape(-1, 2))
+    rep, nmp = np.zeros(n + 1, np.int32), np.zeros(n + 1, np.int32)
+    mpos = np.zeros(int(mz_off[-1]) + 1, np.uint32)
+    a, a_off = C.c_void_p(), C.c_void_p()
+    if L.wm_seed_batch(len(keys), _p(keys, u64p), _p(pos_off, u64p), _p(pos, u64p), n_seq, _p(seq_len, u32p), _p(name_rank, u32p), n,
+                       _p(mz, u64p), _p(mz_off, i64p), _p(qlen, i32p), None if sk is None else _p(sk, u32p), int(max_occ), int(bool(heap)),
+                       C.byref(a), C.byref(a_off), _p(rep, i32p), _p(nmp, i32p), _p(mpos, u32p)) != 0:
+        raise ValueError("wm_seed_batch failed")
+    o = np.ctypeslib.as_array(C.cast(a_off, i64p), shape=(n + 1,)).copy()
+    tot = int(o[-1])
+    xy = np.ctypeslib.as_array(C.cast(a, u64p), shape=(max(tot, 1) * 2,)).copy()[: tot * 2].reshape(-1, 2)
+    _libc.free(a)
+    _libc.free(a_off)
+    return [(xy[o[i]: o[i + 1]].copy(), int(rep[i]), int(nmp[i]), mpos[mz_off[i]: mz_off[i + 1]].copy()) for i in range(n)]
+
+
+HEAP_STAT_NAMES = ("tasks", "anchors", "clocks", "global_heaps", "mismatches")
+
+
+def seed_heap_stats(reset=False):
+    """Counters of the heap merge on the current device (wm_seed_heap_stats), as a dict of HEAP_STAT_NAMES."""
+    L = lib()
+    L.wm_seed_heap_stats.restype = None
+    L.wm_seed_heap_stats.argtypes = [C.POINTER(C.c_double), C.c_int]
+    v = (C.c_double * 5)()
+    L.wm_seed_heap_stats(v, int(bool(reset)))
+    return dict(zip(HEAP_STAT_NAMES, [int(x) for x in v]))
+
+
 class Intv1(C.Structure):
     """mm_idx_intv1_t (reference src/index.c): st, en, max, then score:30 and strand:2 in one int32."""
     _fields_ = [("st", C.c_int32), ("en", C.c_int32), ("max", C.c_int32), ("score", C.c_int32, 30), ("strand", C.c_int32, 2)]

@@ -31,6 +31,7 @@ class MapOpt(C.Structure):  # wm_mapopt_t == mm_mapopt_t (reference src/minimap.
 F_CIGAR, F_OUT_SAM, F_OUT_CG, F_NO_PRINT_2ND, F_PAF_NO_HIT = 0x004, 0x008, 0x020, 0x4000, 0x8000000
 F_NO_DIAG, F_NO_DUAL, F_NO_LJOIN, F_FOR_ONLY, F_REV_ONLY, F_ALL_CHAINS = 0x001, 0x002, 0x400, 0x100000, 0x200000, 0x800000
 F_SPLICE, F_SPLICE_FOR, F_SPLICE_REV, F_SPLICE_FLANK = 0x080, 0x100, 0x200, 0x40000
+F_HEAP_SORT = 0x400000  # MM_F_HEAP_SORT (reference src/minimap.h)
 I_HPC = 0x1  # MM_I_HPC (reference src/minimap.h:41)
 SDUST_MAX_T = 1 << 20  # the largest -T the library takes (csrc/sdust.cuh)
 
@@ -98,7 +99,7 @@ def _check(L, io, mo, spliced_alignment):
 
 
 def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, all_vs_all=False, strand=None, splice=False,
-                 max_intron_len=None, spliced_alignment=False):
+                 max_intron_len=None, spliced_alignment=False, heap_sort=False):
     """mm_set_opt(0) then mm_set_opt(preset) (reference main.c:144-159); -c sets MM_F_OUT_CG|MM_F_CIGAR, -a sets
     MM_F_OUT_SAM|MM_F_CIGAR (main.c).  Self and all-vs-all mapping: no_diag is -D, dual=False is --dual=no, all_vs_all
     is -X (-D -P --no-long-join --dual=no); strand="for" / "rev" is --for-only / --rev-only.  Spliced mapping: the presets
@@ -107,7 +108,9 @@ def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, a
     Spliced base-level alignment (-c / -a with spliced mapping: the two-strand ksw_exts2 rounds, ts:A, N in the CIGAR) is a
     library path that has to be asked for: spliced_alignment=True accepts cigar / sam with spliced mapping, and the -8 that
     wm_check_opt returns for that combination.  Without it, spliced mapping needs cigar=False and sam=False, as the command
-    line does until its refusal is lifted."""
+    line does until its refusal is lifted.  heap_sort=True is --heap-sort=yes: anchors are collected in the order of the
+    reference's heap merge of the occurrence lists (collect_seed_hits_heap), which differs from the default only among anchors
+    with equal reference positions; the command line still refuses it, the library applies it."""
     L = _setup(lib())
     io, mo = IdxOpt(), MapOpt()
     L.wm_set_opt(None, C.byref(io), C.byref(mo))
@@ -134,6 +137,8 @@ def make_options(preset=None, cigar=True, sam=False, no_diag=False, dual=True, a
         if strand not in ("for", "rev", "both"):
             raise ValueError(f"strand must be 'for', 'rev' or 'both', not {strand!r}")
         mo.flag |= {"for": F_FOR_ONLY, "rev": F_REV_ONLY, "both": 0}[strand]
+    if heap_sort:
+        mo.flag |= F_HEAP_SORT
     _check(L, io, mo, spliced_alignment)
     return io, mo
 
@@ -158,11 +163,12 @@ class Mapper:
     before seeding, in every stage; 0 (the default) is off.  The command line still refuses -T; the library applies it.
     junc_bed is --junc-bed: a BED file (plain or gzip) of known introns (BED12 blocks, or one interval per line), read into every
     index part after the index is built.  With spliced_alignment=True every splice DP then adds junc_bonus (self.mo.junc_bonus;
-    9 under splice / cdna, 5 under splice:hq) at annotated donors and acceptors; other mapping is unchanged, as in the reference."""
+    9 under splice / cdna, 5 under splice:hq) at annotated donors and acceptors; other mapping is unchanged, as in the reference.
+    heap_sort=True is --heap-sort=yes (make_options): every stage collects its anchors in the order of the reference's heap merge."""
 
     def __init__(self, ref, kmer_freq=None, preset="map-ont", cigar=True, device=0, n_threads=None, blob=None, sam=False, hpc=False,
                  no_diag=False, dual=True, all_vs_all=False, strand=None, distinct=None, part_bases=None, split=False, mid_occ_frac=None,
-                 splice=False, max_intron_len=None, spliced_alignment=False, sdust_thres=0, junc_bed=None):
+                 splice=False, max_intron_len=None, spliced_alignment=False, sdust_thres=0, junc_bed=None, heap_sort=False):
         if kmer_freq is not None and distinct is not None:
             raise ValueError("give either a -W file (kmer_freq) or distinct=, not both")
         if distinct is not None and not 0.0 < distinct <= 1.0:
@@ -175,7 +181,8 @@ class Mapper:
             raise ValueError(f"sdust_thres must be in 0..{SDUST_MAX_T}, not {sdust_thres!r}")
         self.L = _setup(lib())
         self.io, self.mo = make_options(preset, cigar, sam, no_diag=no_diag, dual=dual, all_vs_all=all_vs_all, strand=strand,
-                                        splice=splice, max_intron_len=max_intron_len, spliced_alignment=spliced_alignment)
+                                        splice=splice, max_intron_len=max_intron_len, spliced_alignment=spliced_alignment,
+                                        heap_sort=heap_sort)
         if hpc:
             self.io.flag |= I_HPC
         if mid_occ_frac is not None:
